@@ -5,6 +5,8 @@ There is NO fallback: if the library is missing or a call fails, a RuntimeError 
 import ctypes
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmonodetr_b200.so")
 _lib = None
@@ -102,6 +104,31 @@ def check(rc: int, what: str = ""):
 
 # number of kernels of THIS library launched so far in this process (bench.py reports the per-step delta)
 _launches = 0
+
+
+def _device_ptr(t, name):
+    if t is None:
+        return None
+    if not t.is_cuda:
+        raise RuntimeError(f"monodetr_b200 {name}: CUDA tensors required (there is no CPU path)")
+    return t.data_ptr()
+
+
+def call(name: str, *args, launches: int = 1):
+    """Run the entry point `name` on the current CUDA stream (appended as the last argument) and count `launches` kernels.
+
+    A tensor argument becomes its device pointer, None becomes NULL and a list / tuple of tensors (entries may be None)
+    becomes a host array of device pointers; anything else is passed as it is.  A tensor that is not on the GPU raises
+    RuntimeError before anything is launched; a non-zero status raises RuntimeError naming the entry point."""
+    conv = []
+    for a in args:
+        if isinstance(a, torch.Tensor) or a is None:
+            a = _device_ptr(a, name)
+        elif isinstance(a, (list, tuple)):
+            a = (c_void_p * len(a))(*[_device_ptr(t, name) for t in a])
+        conv.append(a)
+    check(getattr(lib(), name)(*conv, torch.cuda.current_stream().cuda_stream), name)
+    count(launches)
 
 
 def count(n: int = 1):

@@ -23,10 +23,6 @@ from .position_encoding import build_position_encoding
 _STAGES = [("layer1", 64, 3, 1), ("layer2", 128, 4, 2), ("layer3", 256, 6, 2), ("layer4", 512, 3, 2)]
 
 
-def _s():
-    return torch.cuda.current_stream().cuda_stream
-
-
 class FrozenBatchNorm2d(nn.Module):
     """Buffers only (never trained): y = x * scale + shift with scale = w * rsqrt(rv + eps) (reference :54-64)."""
 
@@ -98,7 +94,6 @@ class _ResNetFn(Function):
 
     @staticmethod
     def forward(ctx, images, meta, *tensors):
-        L = _lib.lib()
         nconv = meta["nconv"]
         weights = tensors[:nconv]
         scales = tensors[nconv:2 * nconv]
@@ -108,12 +103,10 @@ class _ResNetFn(Function):
         # ---- stem (frozen) --------------------------------------------------------------------------------
         H1, W1 = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
         y = torch.empty((B, H1, W1, 64), dtype=torch.float32, device=dev)
-        _lib.check(L.mdb_stem_conv7x7_bn_relu_f32(images.contiguous().data_ptr(), weights[0].contiguous().data_ptr(),
-                                                  scales[0].data_ptr(), shifts[0].data_ptr(), y.data_ptr(), B, H, W, _s()), "stem")
+        _lib.call("mdb_stem_conv7x7_bn_relu_f32", images.contiguous(), weights[0].contiguous(), scales[0], shifts[0], y, B, H, W)
         H2, W2 = (H1 + 2 - 3) // 2 + 1, (W1 + 2 - 3) // 2 + 1
         x = torch.empty((B, H2, W2, 64), dtype=torch.float32, device=dev)
-        _lib.check(L.mdb_maxpool3x3s2_nhwc_f32(y.data_ptr(), x.data_ptr(), B, H1, W1, 64, _s()), "maxpool")
-        _lib.count(2)
+        _lib.call("mdb_maxpool3x3s2_nhwc_f32", y, x, B, H1, W1, 64)
         del y
         # ---- bottlenecks ----------------------------------------------------------------------------------
         saved, packed, feats = [], [], []

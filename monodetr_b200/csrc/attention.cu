@@ -23,6 +23,7 @@
 #include <stdint.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 #include "rng.cuh"
 #include "tc_common.cuh"
 
@@ -544,21 +545,6 @@ constexpr int kFwdSmem = 4 * kTileBytes + 2 * STG * 4 + BC;
 constexpr int kDqSmem = 4 * kTileBytes + 2 * STG * 4 + BC;
 constexpr int kDkvSmem = 5 * kTileBytes + 2 * STG * 4 + 2 * BC * 4;
 
-// The dynamic shared-memory limit is a per (function, device) attribute: several devices per process.
-int set_smem_attributes() {
-    static bool attr_set[64] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
-    if (!attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDqSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_dkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDkvSmem);
-        if (e != cudaSuccess) return (int)e;
-        attr_set[dev] = true;
-    }
-    return 0;
-}
-
 int check(const AttnParams& p) {
     if (p.B <= 0 || p.H <= 0 || p.Lq <= 0 || p.Lk <= 0) return MDB_EINVAL;
     if ((p.ldq | p.ldk | p.ldv | p.ldo) % 4) return MDB_EINVAL;
@@ -586,8 +572,8 @@ int mdb_attention_forward_f32(const float* q, const float* k, const float* v, co
     int rc = check(p);
     if (rc) return rc;
     dim3 grid((Lq + BR - 1) / BR, H, B);
-    rc = set_smem_attributes();
-    if (rc) return rc;
+    const cudaError_t e = set_max_dynamic_smem(attn_fwd_kernel, kFwdSmem);
+    if (e != cudaSuccess) return (int)e;
     attn_fwd_kernel<<<grid, ATT_THREADS, kFwdSmem, static_cast<cudaStream_t>(stream)>>>(p);
     return (int)cudaGetLastError();
 }
@@ -611,8 +597,9 @@ int mdb_attention_backward_f32(const float* q, const float* k, const float* v, c
     if ((lddq | lddk | lddv) % 4) return MDB_EINVAL;
     const long long n = (long long)B * Lq * H;
     attn_delta_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p);
-    rc = set_smem_attributes();
-    if (rc) return rc;
+    cudaError_t e = set_max_dynamic_smem(attn_bwd_dq_kernel, kDqSmem);
+    if (e == cudaSuccess) e = set_max_dynamic_smem(attn_bwd_dkv_kernel, kDkvSmem);
+    if (e != cudaSuccess) return (int)e;
     attn_bwd_dq_kernel<<<dim3((Lq + BR - 1) / BR, H, B), ATT_THREADS, kDqSmem, stream>>>(p);
     attn_bwd_dkv_kernel<<<dim3((Lk + BR - 1) / BR, H, B), ATT_THREADS, kDkvSmem, stream>>>(p);
     return (int)cudaGetLastError();

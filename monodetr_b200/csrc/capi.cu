@@ -1,7 +1,45 @@
-// capi.cu -- ABI version and error strings of libmonodetr_b200.so (see include/monodetr_b200.h).
+// capi.cu -- ABI version and error strings of libmonodetr_b200.so (see include/monodetr_b200.h), and the per-device state of
+// the launch helpers (launch.cuh).
 #include <cuda_runtime.h>
 
+#include <map>
+#include <mutex>
+#include <utility>
+
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
+
+namespace mdb {
+
+namespace {
+std::mutex g_launch_mutex;    // several host threads may launch at once (nn.DataParallel)
+}
+
+int num_sms() {
+    constexpr int kFallback = 132;    // H100 SXM, if the device cannot be queried
+    static std::map<int, int> sms;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return kFallback;
+    std::lock_guard<std::mutex> lock(g_launch_mutex);
+    int& n = sms[dev];
+    if (n == 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = kFallback;
+    return n;
+}
+
+cudaError_t set_max_dynamic_smem(const void* func, int bytes) {
+    static std::map<std::pair<const void*, int>, int> configured;    // the attribute is per (function, device)
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> lock(g_launch_mutex);
+    int& done = configured[{func, dev}];
+    if (done == bytes) return cudaSuccess;
+    e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) done = bytes;
+    return e;
+}
+
+}  // namespace mdb
 
 extern "C" {
 

@@ -22,6 +22,7 @@
 #include <string.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 #include "tc_common.cuh"
 #include "tma_host.cuh"
 
@@ -422,11 +423,9 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
 int g_precision = 2;
 
 // Everything that belongs to ONE device lives here, keyed by cudaGetDevice() (several devices per process: nn.DataParallel,
-// tools/train_val.py:50-55): SM count, the split-K scratch registered by the caller, and (in launch_tc) the per-kernel
-// max-dynamic-smem attribute, which is a per-device property of a function.
+// tools/train_val.py:50-55): the split-K scratch registered by the caller.
 constexpr int kMaxDevices = 64;
 struct DeviceState {
-    int sms = 0;
     float* ws = nullptr;         // split-K scratch: owned by the CALLER (mdb_set_workspace), never freed / reallocated here
     size_t ws_bytes = 0;
 };
@@ -438,16 +437,6 @@ int current_device() {
     return dev;
 }
 
-int num_sms_tc() {
-    DeviceState& d = g_dev[current_device()];
-    if (d.sms == 0) {
-        int dev = 0, sms = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
-        d.sms = sms;
-    }
-    return d.sms;
-}
-
 // `grid` carries the logical tile counts (x = column tiles, y = row tiles, z = split-K slices); the kernel is
 // launched persistent with min(total_tiles, SMs) CTAs.
 template <int BN, int STAGES, int MODE, bool B_MN, int PREC>
@@ -456,18 +445,13 @@ int launch_tc(const CUtensorMap& a, const CUtensorMap& b, TcParams p, dim3 grid,
     constexpr int smem = STAGES * (kTileABytes + BN * 128) + (convb ? (PREC == 1 ? 2 : 1) * BN * 128 : 0) +
                          1024 /*align slack*/ + 256 /*barriers*/;
     static_assert(smem <= 227 * 1024, "dynamic shared memory budget");
-    static bool configured[kMaxDevices] = {};                     // the attribute is per (function, device)
     auto kern = tc_conv_gemm_kernel<BN, STAGES, MODE, B_MN, PREC>;
-    const int dev = current_device();
-    if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return (int)e;
-        configured[dev] = true;
-    }
+    const cudaError_t e = set_max_dynamic_smem(kern, smem);
+    if (e != cudaSuccess) return (int)e;
     p.n_tiles_n = (int)grid.x;
     p.n_tiles_m = (int)grid.y;
     p.total_tiles = (int)(grid.x * grid.y * grid.z);
-    int ctas = num_sms_tc();
+    int ctas = num_sms();
     if (ctas > p.total_tiles) ctas = p.total_tiles;
     if (ctas < 1) return 0;
     // Launch as a PROGRAMMATIC DEPENDENT of the previous kernel in the stream (CUDA >= 11.8, graph capture >= 12.3; MDB_NO_PDL=1: plain launch): the
@@ -583,7 +567,7 @@ namespace {
 // the SMs busy for 0.3 ms).  Returns the number of slices (0 = no split-K).
 int forward_splitk_slices(int precision, int tiles, int kblocks, int bn, bool plain_epilogue, int Cout, long long out_elems) {
     const int kb_per_slice = 32;
-    if (precision == 0 || bn != 128 || tiles * 2 > num_sms_tc() || kblocks < 256 || !plain_epilogue || Cout % 4) return 0;
+    if (precision == 0 || bn != 128 || tiles * 2 > num_sms() || kblocks < 256 || !plain_epilogue || Cout % 4) return 0;
     const int slices = (kblocks + kb_per_slice - 1) / kb_per_slice;
     return (out_elems * slices < (1ll << 31)) ? slices : 0;
 }
@@ -675,9 +659,8 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
             rc = launch_fwd(ma, mb, p, grid, 128, precision, stream);
             if (rc) return rc;
             const long long n4 = out_elems / 4;
-            const int blocks = (int)((n4 + 255) / 256 > 1184 ? 1184 : (n4 + 255) / 256);
-            splitk_reduce_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const float4*>(ws), reinterpret_cast<const float4*>(bias),
-                                                             reinterpret_cast<float4*>(y), n4, Cout / 4, slices, n4);
+            splitk_reduce_kernel<<<grid_cap(n4, 256, num_sms() * 8), 256, 0, stream>>>(
+                reinterpret_cast<const float4*>(ws), reinterpret_cast<const float4*>(bias), reinterpret_cast<float4*>(y), n4, Cout / 4, slices, n4);
             return (int)cudaGetLastError();
         }
     }
@@ -849,7 +832,7 @@ int mdb_conv2d_wgrad_bias_f32(const float* dy, const float* x, const float* rows
     // 128 x BN atomic epilogue stays a small fraction of the work.  Small problems (decoder / head linears, M = 4400 rows
     // = 138 steps): the launch is latency-bound, so spread it over up to one wave with >= 8 steps per CTA (measured
     // 23 us -> ~10 us per launch, ~200 such launches per step).
-    const int sms = num_sms_tc();
+    const int sms = num_sms();
     int big = (2 * sms + tiles - 1) / tiles, small = sms / tiles;
     if (big > total_red / 24) big = total_red / 24;
     if (small > total_red / 8) small = total_red / 8;

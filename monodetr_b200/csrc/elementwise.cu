@@ -5,8 +5,11 @@
 #include <stdint.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 
 namespace {
+
+using namespace mdb;
 
 __global__ void pack_weight_kernel(const float* __restrict__ w, const float* __restrict__ scale, float* __restrict__ out,
                                    int O, int I, int taps, int round_tf32_out) {
@@ -192,7 +195,7 @@ int mdb_pack_conv_weight_f32(const float* w_oihw, const float* scale, float* w_p
                              void* stream) {
     if (!w_oihw || !w_packed || O <= 0 || I <= 0 || taps <= 0) return MDB_EINVAL;
     const long long n = (long long)O * I * taps;
-    const int grid = (int)((n + 255) / 256 > 132 * 16 ? 132 * 16 : (n + 255) / 256);
+    const int grid = grid_cap(n, 256, num_sms() * 16);
     pack_weight_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(w_oihw, scale, w_packed, O, I, taps,
                                                                              mdb_get_precision() == 0);
     return (int)cudaGetLastError();
@@ -202,7 +205,7 @@ int mdb_unpack_conv_wgrad_f32(const float* dw_packed, float* dw_oihw, int O, int
                               void* stream) {
     if (!dw_packed || !dw_oihw || O <= 0 || I <= 0 || taps <= 0) return MDB_EINVAL;
     const long long n = (long long)O * I * taps;
-    const int grid = (int)((n + 255) / 256 > 132 * 16 ? 132 * 16 : (n + 255) / 256);
+    const int grid = grid_cap(n, 256, num_sms() * 16);
     unpack_wgrad_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(dw_packed, dw_oihw, O, I, taps, accumulate);
     return (int)cudaGetLastError();
 }
@@ -284,7 +287,7 @@ int mdb_colsum_f32(const float* x, float* out, long long M, int N, int accumulat
     if (M == 0) return 0;
     const int gx = (N + 31) / 32;
     int gy = (int)((M + 511) / 512);
-    const int cap = (132 * 8 + gx - 1) / gx;
+    const int cap = (num_sms() * 8 + gx - 1) / gx;
     if (gy > cap) gy = cap;
     if (gy < 1 || mdb_get_deterministic()) gy = 1;      // reproducible mode: one accumulation per column
     const int rows = (int)((M + gy - 1) / gy);
@@ -438,12 +441,6 @@ __global__ void maxpool3x3s2_kernel(const float* __restrict__ x, float* __restri
     }
 }
 
-int ew_grid2(long long n, int threads) {
-    long long g = (n + threads - 1) / threads;
-    if (g > 132 * 16) g = 132 * 16;
-    return (int)(g < 1 ? 1 : g);
-}
-
 }  // namespace
 
 extern "C" {
@@ -452,7 +449,7 @@ extern "C" {
 int mdb_relu_backward_f32(const float* dy, const float* y, float* out, long long n, float scale, void* stream) {
     if (!dy || !y || !out || n < 0 || n % 4) return MDB_EINVAL;
     if (n == 0) return 0;
-    relu_bwd_kernel<<<ew_grid2(n / 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    relu_bwd_kernel<<<grid_cap(n / 4, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<const float4*>(dy), reinterpret_cast<const float4*>(y), reinterpret_cast<float4*>(out), n / 4, scale);
     return (int)cudaGetLastError();
 }
@@ -462,7 +459,7 @@ int mdb_dropout_f32(const float* x, float* out, long long n, float p, const unsi
                     unsigned long long site, void* stream) {
     if (!x || !out || !seed || n < 0 || n % 4 || p < 0.f || p >= 1.f) return MDB_EINVAL;
     if (n == 0) return 0;
-    dropout_kernel<<<ew_grid2(n / 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    dropout_kernel<<<grid_cap(n / 4, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(out), n / 4, p, seed, site);
     return (int)cudaGetLastError();
 }
@@ -471,7 +468,7 @@ int mdb_dropout_f32(const float* x, float* out, long long n, float p, const unsi
 int mdb_round_tf32_f32(const float* x, float* out, long long n, void* stream) {
     if (!x || !out || n < 0) return MDB_EINVAL;
     if (n == 0) return 0;
-    round_tf32_kernel<<<ew_grid2(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, out, n);
+    round_tf32_kernel<<<grid_cap(n, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, out, n);
     return (int)cudaGetLastError();
 }
 
@@ -482,14 +479,8 @@ int mdb_stem_conv7x7_bn_relu_f32(const float* x, const float* w, const float* sc
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
     const int smem = (147 * ST_C + 3 * ST_IH * ST_IW) * (int)sizeof(float);
-    static bool configured[64] = {};               // per (function, device)
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
-    if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(stem_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return (int)e;
-        configured[dev] = true;
-    }
+    const cudaError_t e = set_max_dynamic_smem(stem_conv_kernel, smem);
+    if (e != cudaSuccess) return (int)e;
     dim3 grid((Wo + ST_TW - 1) / ST_TW, (Ho + ST_TH - 1) / ST_TH, B);
     // single-pass TF32 mode: the consumer is a tensor-core operand that expects round-to-nearest TF32 values
     stem_conv_kernel<<<grid, 256, smem, stream>>>(x, w, scale, bias, y, H, W, Ho, Wo, mdb_get_precision() == 0 ? 1 : 0);
@@ -500,7 +491,7 @@ int mdb_maxpool3x3s2_nhwc_f32(const float* x, float* y, int B, int H, int W, int
     if (!x || !y || B <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 4) return MDB_EINVAL;
     const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
     const long long n4 = (long long)B * Ho * Wo * C / 4;
-    maxpool3x3s2_kernel<<<ew_grid2(n4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, y, B, H, W, C, Ho, Wo);
+    maxpool3x3s2_kernel<<<grid_cap(n4, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, y, B, H, W, C, Ho, Wo);
     return (int)cudaGetLastError();
 }
 

@@ -12,8 +12,11 @@
 #include <stdint.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 
 namespace {
+
+using namespace mdb;
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 
@@ -310,13 +313,6 @@ __global__ void __launch_bounds__(256) sum_mean_sq_bwd_kernel(const __grid_const
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) g[i] = x[i] * s;
 }
 
-int grid1d(long long n, int threads, int cap) {
-    long long b = (n + threads - 1) / threads;
-    if (b > cap) b = cap;
-    if (b < 1) b = 1;
-    return (int)b;
-}
-
 }  // namespace
 
 extern "C" {
@@ -325,7 +321,7 @@ int mdb_box_refine_forward_f32(const float* tmp, const float* ref, float* y, lon
     if (n < 0 || (ref_dim != 2 && ref_dim != 6)) return MDB_EINVAL;
     if (n == 0) return 0;
     if (!tmp || !ref || !y) return MDB_EINVAL;
-    box_refine_fwd_kernel<<<grid1d(n * 6, 256, 1184), 256, 0, static_cast<cudaStream_t>(stream)>>>(tmp, ref, y, n, ref_dim);
+    box_refine_fwd_kernel<<<grid_cap(n * 6, 256, num_sms() * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(tmp, ref, y, n, ref_dim);
     return (int)cudaGetLastError();
 }
 int mdb_box_refine_backward_f32(const float* dy, const float* y, const float* ref, float* dtmp, float* dref, long long n, int ref_dim,
@@ -333,7 +329,7 @@ int mdb_box_refine_backward_f32(const float* dy, const float* y, const float* re
     if (n < 0 || (ref_dim != 2 && ref_dim != 6)) return MDB_EINVAL;
     if (n == 0) return 0;
     if (!dy || !y || !ref || !dtmp) return MDB_EINVAL;
-    box_refine_bwd_kernel<<<grid1d(n * 6, 256, 1184), 256, 0, static_cast<cudaStream_t>(stream)>>>(dy, y, ref, dtmp, dref, n, ref_dim);
+    box_refine_bwd_kernel<<<grid_cap(n * 6, 256, num_sms() * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(dy, y, ref, dtmp, dref, n, ref_dim);
     return (int)cudaGetLastError();
 }
 
@@ -366,8 +362,8 @@ int mdb_depth_tail_forward_f32(const float* logits, const float* bins, const flo
     if (npix < 0 || nb <= 0 || nb > kMaxBins || E <= 0 || C <= 0 || C % 4 || C > 256) return MDB_EINVAL;
     if (npix == 0) return 0;
     if (!logits || !bins || !emb || !wdepth || !ip) return MDB_EINVAL;
-    depth_tail_fwd_kernel<<<grid1d(npix * 32, 256, 1184), 256, 0, static_cast<cudaStream_t>(stream)>>>(logits, bins, emb, wdepth, ip, npix, nb,
-                                                                                                      E, C, dmax);
+    depth_tail_fwd_kernel<<<grid_cap(npix * 32, 256, num_sms() * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(logits, bins, emb, wdepth, ip, npix, nb,
+                                                                                                                  E, C, dmax);
     return (int)cudaGetLastError();
 }
 // demb (E x C) is zero-filled by the call.
@@ -381,16 +377,10 @@ int mdb_depth_tail_backward_f32(const float* logits, const float* bins, const fl
     if (npix == 0) return 0;
     if (!logits || !bins || !emb || !d_ip || !dlogits) return MDB_EINVAL;
     const int smem = E * C * 4;
-    static bool configured[64] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
-    if (!configured[dev]) {
-        e = cudaFuncSetAttribute(depth_tail_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        if (e != cudaSuccess) return (int)e;
-        configured[dev] = true;
-    }
-    depth_tail_bwd_kernel<<<grid1d(npix * 32, 256, 132), 256, smem, stream>>>(logits, bins, emb, d_ip, d_wd_ext, dlogits, demb, npix, nb, E, C,
-                                                                              dmax);
+    e = set_max_dynamic_smem(depth_tail_bwd_kernel, 96 * 1024);
+    if (e != cudaSuccess) return (int)e;
+    depth_tail_bwd_kernel<<<grid_cap(npix * 32, 256, num_sms()), 256, smem, stream>>>(logits, bins, emb, d_ip, d_wd_ext, dlogits, demb, npix, nb, E, C,
+                                                                                       dmax);
     return (int)cudaGetLastError();
 }
 
@@ -398,7 +388,7 @@ int mdb_mean3_f32(const float* a, const float* b, const float* c, float* out, lo
     if (n < 0 || n % 4) return MDB_EINVAL;
     if (n == 0) return 0;
     if (!a || !b || !c || !out) return MDB_EINVAL;
-    mean3_kernel<<<grid1d(n / 4, 256, 1184), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    mean3_kernel<<<grid_cap(n / 4, 256, num_sms() * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<const float4*>(a), reinterpret_cast<const float4*>(b), reinterpret_cast<const float4*>(c), reinterpret_cast<float4*>(out), n / 4);
     return (int)cudaGetLastError();
 }
@@ -406,7 +396,7 @@ int mdb_scale_f32(const float* a, float* out, long long n, float s, void* stream
     if (n < 0 || n % 4) return MDB_EINVAL;
     if (n == 0) return 0;
     if (!a || !out) return MDB_EINVAL;
-    scale_kernel<<<grid1d(n / 4, 256, 1184), 256, 0, static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float4*>(a),
+    scale_kernel<<<grid_cap(n / 4, 256, num_sms() * 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const float4*>(a),
                                                                                          reinterpret_cast<float4*>(out), n / 4, s);
     return (int)cudaGetLastError();
 }
@@ -426,7 +416,7 @@ int mdb_sum_mean_squares_forward_f32(int count, const float* const* x, const lon
         tb.x[k] = x[k]; tb.g[k] = nullptr; tb.n[k] = n[k];
         if (n[k] > nmax) nmax = n[k];
     }
-    sum_mean_sq_fwd_kernel<<<dim3(grid1d(nmax, 256 * 8, 64), count), 256, 0, stream>>>(tb, loss);
+    sum_mean_sq_fwd_kernel<<<dim3(grid_cap(nmax, 256 * 8, 64), count), 256, 0, stream>>>(tb, loss);
     return (int)cudaGetLastError();
 }
 int mdb_sum_mean_squares_backward_f32(int count, const float* const* x, float* const* g, const long long* n, const float* dloss,
@@ -441,7 +431,7 @@ int mdb_sum_mean_squares_backward_f32(int count, const float* const* x, float* c
         tb.x[k] = x[k]; tb.g[k] = g[k]; tb.n[k] = n[k];
         if (n[k] > nmax) nmax = n[k];
     }
-    sum_mean_sq_bwd_kernel<<<dim3(grid1d(nmax, 256 * 4, 128), count), 256, 0, static_cast<cudaStream_t>(stream_)>>>(tb, dloss);
+    sum_mean_sq_bwd_kernel<<<dim3(grid_cap(nmax, 256 * 4, 128), count), 256, 0, static_cast<cudaStream_t>(stream_)>>>(tb, dloss);
     return (int)cudaGetLastError();
 }
 

@@ -20,11 +20,13 @@
 // Generic path (any D/L/P, fp32 and fp64): one warp per unit, lanes stride over channels.
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 
 namespace {
+
+using namespace mdb;
 
 constexpr int kMaxLevels = 8;
 constexpr int kThreads = 256;
@@ -54,16 +56,15 @@ __device__ __forceinline__ double floor_t(double a) { return floor(a); }
 // strip of horizontally adjacent pixels), and its 8 warps walk it side by side, so that the bilinear footprints of
 // neighbouring queries are re-read from the SM's L1 instead of L2 (an interleaved grid-stride walk spreads a strip over
 // all SMs and gets ~35 % L1 hits; the contiguous walk reuses a line across ~8 neighbouring queries).
-template <int LPU, int LT /*compile-time level count, 0 = runtime*/>
+template <int LPU>
 __global__ void __launch_bounds__(kThreads)
 msda_fwd_vec_kernel(const float* __restrict__ value, const int64_t* __restrict__ shapes,
                     const int64_t* __restrict__ lsi, const float* __restrict__ loc,
-                    const float* __restrict__ attn, int S, int M, int L_rt, int Lq, long long n_units,
+                    const float* __restrict__ attn, int S, int M, int L, int Lq, long long n_units,
                     long long units_per_block, float* __restrict__ out) {
     constexpr int D = 4 * LPU;
     constexpr int UPW = 32 / LPU;
     constexpr int P = 4;
-    const int L = LT ? LT : L_rt;
     __shared__ LevelInfo lv;
     if (threadIdx.x < L) {
         lv.H[threadIdx.x] = (int)shapes[2 * threadIdx.x];
@@ -89,8 +90,8 @@ msda_fwd_vec_kernel(const float* __restrict__ value, const int64_t* __restrict__
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 
 #pragma unroll
-        for (int l = 0; l < (LT ? LT : kMaxLevels); ++l) {
-            if (!LT && l >= L) break;
+        for (int l = 0; l < kMaxLevels; ++l) {
+            if (l >= L) break;
             const int H = lv.H[l], W = lv.W[l];
             const float fW = (float)W, fH = (float)H;
             const float* vl = vb + (size_t)lv.start[l] * pix;
@@ -629,22 +630,6 @@ msda_bwd_value_ordered_kernel(const int64_t* __restrict__ shapes, const int64_t*
     }
 }
 
-int num_sms() {
-    static int sms[64] = {};                       // per device
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
-    if (sms[dev] == 0 && cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms[dev] = 132;
-    return sms[dev];
-}
-
-int grid_for(long long n_warps_needed, int blocks_per_sm) {
-    long long blocks = (n_warps_needed + (kThreads / 32) - 1) / (kThreads / 32);
-    const long long cap = (long long)num_sms() * blocks_per_sm;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    return (int)blocks;
-}
-
 int check_common(const void* a, const void* b, const void* c, const void* d, const void* e, int B, int S,
                  int M, int D, int L, int Lq, int P) {
     if (B < 0 || S < 0 || M < 0 || D < 0 || L < 0 || Lq < 0 || P < 0) return MDB_EINVAL;
@@ -672,24 +657,21 @@ int forward_impl(const T* value, const int64_t* shapes, const int64_t* lsi, cons
                           aligned16(loc) && aligned16(attn) && aligned16(out);
         if (fast) {
             const int lpu = D / 4, upw = 32 / lpu;
-            const int grid = grid_for((n_units + upw - 1) / upw, 8);
+            const int grid = grid_cap((n_units + upw - 1) / upw, kThreads / 32, num_sms() * 8);
             const long long per = (kThreads / 32) * upw;                        // units one CTA pass covers
             const long long upb = ((n_units + grid - 1) / grid + per - 1) / per * per;
-            static const bool use_old = getenv("MDB_MSDA_OLD") != nullptr;     // A/B switch for profiling only
-            if (lpu == 8 && L == 4 && use_old)
-                msda_fwd_vec_kernel<8, 4><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, L, Lq, n_units, upb, out);
-            else if (lpu == 8 && L == 4)
+            if (lpu == 8 && L == 4)
                 msda_fwd_d32_kernel<false><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, nullptr, 0, S, M, Lq, n_units, upb, out);
             else if (lpu == 8)
-                msda_fwd_vec_kernel<8, 0><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, L, Lq, n_units, upb, out);
+                msda_fwd_vec_kernel<8><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, L, Lq, n_units, upb, out);
             else if (lpu == 4)
-                msda_fwd_vec_kernel<4, 0><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, L, Lq, n_units, upb, out);
+                msda_fwd_vec_kernel<4><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, L, Lq, n_units, upb, out);
             else
-                msda_fwd_vec_kernel<16, 0><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, L, Lq, n_units, upb, out);
+                msda_fwd_vec_kernel<16><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, L, Lq, n_units, upb, out);
             return (int)cudaGetLastError();
         }
     }
-    const int grid = grid_for(n_units, 8);
+    const int grid = grid_cap(n_units, kThreads / 32, num_sms() * 8);
     msda_fwd_generic_kernel<T><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, S, M, D, L, Lq, P, n_units, out);
     return (int)cudaGetLastError();
 }
@@ -719,7 +701,7 @@ int backward_impl(const T* value, const int64_t* shapes, const int64_t* lsi, con
     if (mdb_get_deterministic()) {
         // grad_loc / grad_attn by the generic kernel (warp reductions, no atomics) with its scatter compiled out, then the
         // value gradient in a fixed accumulation order
-        const int grid = grid_for(n_units, 8);
+        const int grid = grid_cap(n_units, kThreads / 32, num_sms() * 8);
         msda_bwd_generic_kernel<T, false><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, grad_out, S, M, D, L, Lq, P, n_units, grad_value, grad_loc, grad_attn);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return (int)e;
@@ -733,7 +715,7 @@ int backward_impl(const T* value, const int64_t* shapes, const int64_t* lsi, con
                           aligned16(loc) && aligned16(attn) && aligned16(grad_out) && aligned16(grad_value);
         if (fast) {
             const int lpu = D / 4, upw = 32 / lpu;
-            const int grid = grid_for((n_units + upw - 1) / upw, 6);
+            const int grid = grid_cap((n_units + upw - 1) / upw, kThreads / 32, num_sms() * 6);
             const long long per = (kThreads / 32) * upw;
             const long long upb = ((n_units + grid - 1) / grid + per - 1) / per * per;
             // (Two variants were tried on another GPU and removed: a branch-free backward organised like msda_fwd_d32_kernel, and
@@ -747,7 +729,7 @@ int backward_impl(const T* value, const int64_t* shapes, const int64_t* lsi, con
             return (int)cudaGetLastError();
         }
     }
-    const int grid = grid_for(n_units, 8);
+    const int grid = grid_cap(n_units, kThreads / 32, num_sms() * 8);
     msda_bwd_generic_kernel<T><<<grid, kThreads, 0, stream>>>(value, shapes, lsi, loc, attn, grad_out, S, M, D, L, Lq, P, n_units, grad_value, grad_loc, grad_attn);
     return (int)cudaGetLastError();
 }
@@ -785,7 +767,7 @@ int mdb_msda_fused_forward_f32(const float* value, const int64_t* spatial_shapes
     if (n_units == 0) return 0;
     if (!ref || !out) return MDB_EINVAL;
     if (!aligned16(value) || !aligned16(offsets) || !aligned16(logits) || !aligned16(out)) return MDB_EUNSUPPORTED;
-    const int grid = grid_for((n_units + 3) / 4, 8);
+    const int grid = grid_cap((n_units + 3) / 4, kThreads / 32, num_sms() * 8);
     const long long per = (kThreads / 32) * 4;
     const long long upb = ((n_units + grid - 1) / grid + per - 1) / per * per;
     msda_fwd_d32_kernel<true><<<grid, kThreads, 0, static_cast<cudaStream_t>(stream_)>>>(value, spatial_shapes, level_start, offsets, logits, ref,
@@ -811,7 +793,7 @@ int mdb_msda_fused_backward_f32(const float* value, const int64_t* spatial_shape
     }
     if (n_units == 0) return 0;
     if (!ref || !grad_out || !grad_offsets || !grad_logits) return MDB_EINVAL;
-    const int grid = grid_for((n_units + 3) / 4, 6);
+    const int grid = grid_cap((n_units + 3) / 4, kThreads / 32, num_sms() * 6);
     const long long per = (kThreads / 32) * 4;
     const long long upb = ((n_units + grid - 1) / grid + per - 1) / per * per;
     msda_bwd_vec_kernel<8, 4, true><<<grid, kThreads, 0, stream>>>(value, spatial_shapes, level_start, offsets, logits, grad_out, S, M, Lq, n_units,
@@ -937,9 +919,7 @@ int mdb_msda_prep_forward_f32(const float* off, const float* logits, const float
     if (L * P > kPrepMaxLP || (L * P) % 4 || P % 2 || (ref_dim != 2 && ref_dim != 6)) return MDB_EUNSUPPORTED;
     const long long n = (long long)B * Lq * M;
     if (n == 0) return 0;
-    long long g = (n + 255) / 256;
-    if (g > 132 * 16) g = 132 * 16;
-    msda_prep_fwd_kernel<<<(int)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(off, logits, ref, spatial_shapes, M, L, P, ref_dim, n, loc, attn);
+    msda_prep_fwd_kernel<<<grid_cap(n, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(off, logits, ref, spatial_shapes, M, L, P, ref_dim, n, loc, attn);
     return (int)cudaGetLastError();
 }
 
@@ -950,9 +930,7 @@ int mdb_msda_prep_backward_f32(const float* dloc, const float* dattn, const floa
     if (L * P > kPrepMaxLP || (L * P) % 4 || P % 2 || (ref_dim != 2 && ref_dim != 6)) return MDB_EUNSUPPORTED;
     const long long n = (long long)B * Lq * M;
     if (n == 0) return 0;
-    long long g = (n + 255) / 256;
-    if (g > 132 * 16) g = 132 * 16;
-    msda_prep_bwd_kernel<<<(int)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(dloc, dattn, attn, ref, spatial_shapes, M, L, P, ref_dim, n, doff, dlogits);
+    msda_prep_bwd_kernel<<<grid_cap(n, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(dloc, dattn, attn, ref, spatial_shapes, M, L, P, ref_dim, n, doff, dlogits);
     return (int)cudaGetLastError();
 }
 

@@ -7,9 +7,12 @@
 #include <stdint.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 #include "rng.cuh"
 
 namespace {
+
+using namespace mdb;
 
 constexpr int LN_THREADS = 256;      // 8 warps = 8 rows per CTA iteration
 constexpr int LN_MAXV = 8;           // float4 vectors per lane -> C <= 1024
@@ -330,12 +333,6 @@ gn_bwd_apply_kernel(const float* __restrict__ dy, const float* __restrict__ x, c
     }
 }
 
-int ew_grid(long long n, int threads) {
-    long long g = (n + threads - 1) / threads;
-    if (g > 132 * 16) g = 132 * 16;
-    return (int)(g < 1 ? 1 : g);
-}
-
 }  // namespace
 
 extern "C" {
@@ -348,7 +345,7 @@ int mdb_add_layernorm_forward_f32(const float* x, const float* res, const float*
     if (drop_p > 0.f && !seed) return MDB_EINVAL;
     if (M == 0) return 0;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const int grid = ew_grid(M, LN_THREADS / 32);
+    const int grid = grid_cap(M, LN_THREADS / 32, num_sms() * 16);
 #define MDB_LN_FWD(NV) add_ln_fwd_kernel<NV><<<grid, LN_THREADS, 0, stream>>>(x, res, gamma, beta, y, mean, rstd, M, eps, drop_p, seed, site)
     switch (C / 128) {
         case 1: MDB_LN_FWD(1); break;
@@ -376,8 +373,7 @@ int mdb_add_layernorm_backward_f32(const float* dy, const float* x, const float*
         cudaMemsetAsync(dbeta, 0, sizeof(float) * C, stream);
     }
     if (M == 0) return 0;
-    int grid = ew_grid(M, LN_THREADS / 32);
-    if (grid > 132 * 4) grid = 132 * 4;
+    const int grid = grid_cap(M, LN_THREADS / 32, num_sms() * 4);
 #define MDB_LN_BWD(NV) add_ln_bwd_kernel<NV><<<grid, LN_THREADS, 0, stream>>>(dy, x, res, gamma, mean, rstd, dx, dres, dgamma, dbeta, M, drop_p, seed, site)
     switch (C / 128) {
         case 1: MDB_LN_BWD(1); break;
@@ -400,7 +396,7 @@ int mdb_groupnorm_forward_f32(const float* x, const float* gamma, const float* b
     if (blocks > 64) blocks = 64;
     const int ppb = (HW + blocks - 1) / blocks;
     gn_stats_kernel<<<dim3((HW + ppb - 1) / ppb, B), GN_THREADS, 0, stream>>>(x, stats_ws, HW, C, G, ppb);
-    gn_apply_kernel<<<ew_grid((long long)B * HW * C / 4, GN_THREADS), GN_THREADS, 0, stream>>>(x, stats_ws, gamma, beta, y,
+    gn_apply_kernel<<<grid_cap((long long)B * HW * C / 4, GN_THREADS, num_sms() * 16), GN_THREADS, 0, stream>>>(x, stats_ws, gamma, beta, y,
                                                                                                  mean, rstd, B, HW, C, G, eps, relu);
     return (int)cudaGetLastError();
 }
@@ -421,7 +417,7 @@ int mdb_groupnorm_backward_f32(const float* dy, const float* x, const float* y, 
     const int ppb = (HW + blocks - 1) / blocks;
     gn_bwd_stats_kernel<<<dim3((HW + ppb - 1) / ppb, B), GN_THREADS, 0, stream>>>(dy, x, y, gamma, mean, rstd, stats_ws, dgamma,
                                                                                   dbeta, HW, C, G, ppb, relu);
-    gn_bwd_apply_kernel<<<ew_grid((long long)B * HW * C / 4, GN_THREADS), GN_THREADS, 0, stream>>>(dy, x, y, gamma, mean, rstd,
+    gn_bwd_apply_kernel<<<grid_cap((long long)B * HW * C / 4, GN_THREADS, num_sms() * 16), GN_THREADS, 0, stream>>>(dy, x, y, gamma, mean, rstd,
                                                                                                     stats_ws, dx, B, HW, C, G, relu);
     return (int)cudaGetLastError();
 }

@@ -17,6 +17,7 @@
 #include <stdint.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 
 namespace {
 
@@ -62,12 +63,8 @@ extern "C" int mdb_adamw_step_f32(float* p, const float* g, float* m, float* v, 
     if (!p || !g || !m || !v) return MDB_EINVAL;
     if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15u)
         return MDB_EINVAL;
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    long long blocks = (n / 4 + 255) / 256;
-    if (blocks > (long long)sms * 8) blocks = (long long)sms * 8;
-    if (blocks < 1) blocks = 1;
-    adamw_flat_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(p, g, m, v, n, n_decay, beta1, one_minus_beta1, beta2,
+    const int blocks = mdb::grid_cap(n / 4, 256, mdb::num_sms() * 8);
+    adamw_flat_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(p, g, m, v, n, n_decay, beta1, one_minus_beta1, beta2,
                                                                                        one_minus_beta2, eps, weight_decay, step_size,
                                                                                        step_size_dev);
     return (int)cudaGetLastError();

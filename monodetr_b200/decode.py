@@ -18,10 +18,6 @@ DET_COLS = 37
 OUT_COLS = 14
 
 
-def _stream(t):
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
 def _f32(t, device):
     if not isinstance(t, torch.Tensor):
         t = torch.as_tensor(np.asarray(t, dtype=np.float32))
@@ -43,9 +39,7 @@ def extract_dets_from_outputs(outputs, K=50, topk=50):
         raise ValueError("extract_dets_from_outputs: head outputs with unexpected shapes")
     dets = torch.empty(B, topk, DET_COLS, device=dev, dtype=torch.float32)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().mdb_extract_dets_f32(logits.data_ptr(), boxes.data_ptr(), dim3.data_ptr(), depth.data_ptr(),
-                                                   angle.data_ptr(), B, Q, C, topk, dets.data_ptr(), _stream(dets)),
-                   "mdb_extract_dets_f32")
+        _lib.call("mdb_extract_dets_f32", logits, boxes, dim3, depth, angle, B, Q, C, topk, dets)
     return dets
 
 
@@ -72,9 +66,7 @@ def decode_detections_device(dets, img_size, calibs, cls_mean_size, threshold):
     rows = torch.empty(B, topk, OUT_COLS, device=dev, dtype=torch.float32)
     count = torch.empty(B, device=dev, dtype=torch.int32)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().mdb_decode_dets_f32(dets.data_ptr(), img_size.data_ptr(), P2.data_ptr(), mean.data_ptr(), B, topk,
-                                                  mean.shape[0], float(threshold), rows.data_ptr(), count.data_ptr(), _stream(rows)),
-                   "mdb_decode_dets_f32")
+        _lib.call("mdb_decode_dets_f32", dets, img_size, P2, mean, B, topk, mean.shape[0], float(threshold), rows, count)
     return rows, count
 
 

@@ -15,14 +15,6 @@ from . import _lib, kernels as K, tc
 from .msda import MSDeformAttnFunction
 
 
-def _s():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _p(t):
-    return 0 if t is None else t.data_ptr()
-
-
 def _pad4(n):
     return (n + 3) // 4 * 4
 
@@ -98,8 +90,7 @@ class Branch:
 def relu_backward(dy, y, scale=1.0):
     dy = dy.contiguous()
     out = torch.empty_like(dy)
-    _lib.check(_lib.lib().mdb_relu_backward_f32(_p(dy), _p(y), _p(out), dy.numel(), float(scale), _s()), "relu_backward")
-    _lib.count(1)
+    _lib.call("mdb_relu_backward_f32", dy, y, out, dy.numel(), float(scale))
     return out
 
 
@@ -107,8 +98,7 @@ def dropout_raw(x, p, site, seed=None):
     x = x.contiguous()
     out = torch.empty_like(x)
     seed = seed if seed is not None else K.seed_tensor(x.device)
-    _lib.check(_lib.lib().mdb_dropout_f32(_p(x), _p(out), x.numel(), float(p), _p(seed), site, _s()), "dropout")
-    _lib.count(1)
+    _lib.call("mdb_dropout_f32", x, out, x.numel(), float(p), seed, site)
     return out
 
 
@@ -349,9 +339,7 @@ class _MsdaPrep(Function):
         rd = refc.shape[-1]
         loc = torch.empty((B, Lq, M, L, P, 2), dtype=torch.float32, device=off.device)
         attn = torch.empty((B, Lq, M, L, P), dtype=torch.float32, device=off.device)
-        _lib.check(_lib.lib().mdb_msda_prep_forward_f32(_p(off), _p(logits), _p(refc), _p(shapes), B, Lq, M, L, P, rd, _p(loc),
-                                                        _p(attn), _s()), "msda_prep_forward")
-        _lib.count(1)
+        _lib.call("mdb_msda_prep_forward_f32", off, logits, refc, shapes, B, Lq, M, L, P, rd, loc, attn)
         # 6-d reference boxes that require grad (not on the model path, where they are detached -- depthaware_transformer.py
         # :613 -- but a custom decoder may pass them): keep the offsets for the box gradient
         keep_off = rd == 6 and ref.requires_grad
@@ -368,9 +356,7 @@ class _MsdaPrep(Function):
         dattn = dattn.contiguous()
         doff = torch.empty(oshape, dtype=torch.float32, device=dloc.device)
         dlogits = torch.empty(lshape, dtype=torch.float32, device=dloc.device)
-        _lib.check(_lib.lib().mdb_msda_prep_backward_f32(_p(dloc), _p(dattn), _p(attn), _p(refc), _p(shapes), B, Lq, M, L, P, rd,
-                                                         _p(doff), _p(dlogits), _s()), "msda_prep_backward")
-        _lib.count(1)
+        _lib.call("mdb_msda_prep_backward_f32", dloc, dattn, attn, refc, shapes, B, Lq, M, L, P, rd, doff, dlogits)
         dref = None
         if ctx.needs_input_grad[2]:
             if rd == 2:
@@ -398,12 +384,10 @@ def msda_fused_forward_raw(value, shapes, lsi, off, logits, refc):
     if _m.PROBE is not None:        # bench.py: CUDA events tight around the launch (nothing else between them)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-    _lib.check(_lib.lib().mdb_msda_fused_forward_f32(_p(value), _p(shapes), _p(lsi), _p(off), _p(logits), _p(refc), B, S, M, D, 4, Lq, 4, rd,
-                                                     _p(out), _s()), "msda_fused_forward")
+    _lib.call("mdb_msda_fused_forward_f32", value, shapes, lsi, off, logits, refc, B, S, M, D, 4, Lq, 4, rd, out)
     if _m.PROBE is not None:
         e1.record()
         _m.PROBE.append((e0, e1, B, Lq))
-    _lib.count(1)
     return out
 
 
@@ -412,9 +396,7 @@ def msda_fused_backward_raw(value, shapes, lsi, off, logits, refc, dout):
     Lq, rd = off.shape[1], refc.shape[-1]
     dout = dout.contiguous()
     gv, goff, glog = torch.empty_like(value), torch.empty_like(off), torch.empty_like(logits)
-    _lib.check(_lib.lib().mdb_msda_fused_backward_f32(_p(value), _p(shapes), _p(lsi), _p(off), _p(logits), _p(refc), _p(dout), B, S, M, D, 4, Lq,
-                                                      4, rd, _p(gv), _p(goff), _p(glog), _s()), "msda_fused_backward")
-    _lib.count(1)
+    _lib.call("mdb_msda_fused_backward_f32", value, shapes, lsi, off, logits, refc, dout, B, S, M, D, 4, Lq, 4, rd, gv, goff, glog)
     return gv, goff, glog
 
 
@@ -582,8 +564,7 @@ class _DepthSample(Function):
         B, H, W = depth.shape
         N = xy.shape[1]
         out = torch.empty((B, N), dtype=torch.float32, device=depth.device)
-        _lib.check(_lib.lib().mdb_depth_sample_forward_f32(_p(depth), _p(xy), _p(out), B, H, W, N, _s()), "depth_sample_forward")
-        _lib.count(1)
+        _lib.call("mdb_depth_sample_forward_f32", depth, xy, out, B, H, W, N)
         ctx.save_for_backward(xy)
         ctx.meta = (B, H, W, N)
         return out
@@ -594,8 +575,7 @@ class _DepthSample(Function):
         (xy,) = ctx.saved_tensors
         B, H, W, N = ctx.meta
         dd = torch.empty((B, H, W), dtype=torch.float32, device=dout.device)
-        _lib.check(_lib.lib().mdb_depth_sample_backward_f32(_p(dout.contiguous()), _p(xy), _p(dd), B, H, W, N, _s()), "depth_sample_backward")
-        _lib.count(1)
+        _lib.call("mdb_depth_sample_backward_f32", dout.contiguous(), xy, dd, B, H, W, N)
         return dd, None
 
 
@@ -617,8 +597,7 @@ class _BoxRefine(Function):
         rd = refc.shape[-1]
         n = tmp.numel() // 6
         y = torch.empty_like(tmp)
-        _lib.check(_lib.lib().mdb_box_refine_forward_f32(_p(tmp), _p(refc), _p(y), n, rd, _s()), "box_refine_forward")
-        _lib.count(1)
+        _lib.call("mdb_box_refine_forward_f32", tmp, refc, y, n, rd)
         ctx.save_for_backward(y, refc)
         ctx.meta = (n, rd, ref.shape)
         return y
@@ -631,8 +610,7 @@ class _BoxRefine(Function):
         dy = dy.contiguous()
         dtmp = torch.empty_like(y)
         dref = torch.empty(rshape, dtype=torch.float32, device=y.device) if ctx.needs_input_grad[1] else None
-        _lib.check(_lib.lib().mdb_box_refine_backward_f32(_p(dy), _p(y), _p(refc), _p(dtmp), _p(dref), n, rd, _s()), "box_refine_backward")
-        _lib.count(1)
+        _lib.call("mdb_box_refine_backward_f32", dy, y, refc, dtmp, dref, n, rd)
         return dtmp, dref
 
 
@@ -651,9 +629,7 @@ class _HeadDepth(Function):
         B, N, _ = coord.shape
         _, H, W = wdepth.shape
         out = torch.empty((B, N, 2), dtype=torch.float32, device=coord.device)
-        _lib.check(_lib.lib().mdb_head_depth_forward_f32(_p(coord), _p(size3d), _p(depth_reg), _p(wdepth), _p(calibs), _p(img_sizes), _p(out),
-                                                         B, N, H, W, _s()), "head_depth_forward")
-        _lib.count(1)
+        _lib.call("mdb_head_depth_forward_f32", coord, size3d, depth_reg, wdepth, calibs, img_sizes, out, B, N, H, W)
         ctx.save_for_backward(coord, size3d, depth_reg, calibs, img_sizes)
         ctx.meta = (B, N, H, W)
         return out
@@ -666,9 +642,7 @@ class _HeadDepth(Function):
         dout = dout.contiguous()
         dcoord, dsize, dreg = torch.empty_like(coord), torch.empty_like(size3d), torch.empty_like(depth_reg)
         dwd = torch.empty((B, H, W), dtype=torch.float32, device=dout.device)
-        _lib.check(_lib.lib().mdb_head_depth_backward_f32(_p(dout), _p(coord), _p(size3d), _p(depth_reg), _p(calibs), _p(img_sizes), _p(dcoord),
-                                                          _p(dsize), _p(dreg), _p(dwd), B, N, H, W, _s()), "head_depth_backward")
-        _lib.count(1)
+        _lib.call("mdb_head_depth_backward_f32", dout, coord, size3d, depth_reg, calibs, img_sizes, dcoord, dsize, dreg, dwd, B, N, H, W)
         return dcoord, dsize, dreg, dwd, None, None
 
 
@@ -688,9 +662,7 @@ class _DepthTail(Function):
         E, C = embc.shape
         wd = torch.empty((B, H, W), dtype=torch.float32, device=logits.device)
         ip = torch.empty((B, H, W, C), dtype=torch.float32, device=logits.device)
-        _lib.check(_lib.lib().mdb_depth_tail_forward_f32(_p(logits), _p(bins), _p(embc), _p(wd), _p(ip), B * H * W, nb, E, C, float(dmax), _s()),
-                   "depth_tail_forward")
-        _lib.count(1)
+        _lib.call("mdb_depth_tail_forward_f32", logits, bins, embc, wd, ip, B * H * W, nb, E, C, float(dmax))
         ctx.save_for_backward(logits, bins, embc)
         ctx.meta = (B * H * W, nb, E, C, float(dmax))
         return wd, ip
@@ -704,9 +676,7 @@ class _DepthTail(Function):
         dwd = None if dwd is None else dwd.contiguous()
         dlogits = torch.empty_like(logits)
         demb = torch.empty_like(embc)
-        _lib.check(_lib.lib().mdb_depth_tail_backward_f32(_p(logits), _p(bins), _p(embc), _p(dip), _p(dwd), _p(dlogits), _p(demb), npix, nb, E, C,
-                                                          dmax, _s()), "depth_tail_backward")
-        _lib.count(1)
+        _lib.call("mdb_depth_tail_backward_f32", logits, bins, embc, dip, dwd, dlogits, demb, npix, nb, E, C, dmax)
         return dlogits, None, demb, None
 
 
@@ -719,8 +689,7 @@ class _Mean3(Function):
     def forward(ctx, a, b, c):
         a, b, c = a.contiguous(), b.contiguous(), c.contiguous()
         out = torch.empty_like(a)
-        _lib.check(_lib.lib().mdb_mean3_f32(_p(a), _p(b), _p(c), _p(out), a.numel(), _s()), "mean3")
-        _lib.count(1)
+        _lib.call("mdb_mean3_f32", a, b, c, out, a.numel())
         return out
 
     @staticmethod
@@ -728,8 +697,7 @@ class _Mean3(Function):
     def backward(ctx, dy):
         dy = dy.contiguous()
         g = torch.empty_like(dy)
-        _lib.check(_lib.lib().mdb_scale_f32(_p(dy), _p(g), dy.numel(), 1.0 / 3.0, _s()), "scale")
-        _lib.count(1)
+        _lib.call("mdb_scale_f32", dy, g, dy.numel(), 1.0 / 3.0)
         return g, g, g
 
 
@@ -746,10 +714,8 @@ class _SumMeanSquares(Function):
         xs = [x.contiguous() for x in xs]
         n = len(xs)
         loss = torch.empty((), dtype=torch.float32, device=xs[0].device)
-        ptrs = (_ct.c_void_p * n)(*[x.data_ptr() for x in xs])
         nums = (_ct.c_longlong * n)(*[x.numel() for x in xs])
-        _lib.check(_lib.lib().mdb_sum_mean_squares_forward_f32(n, ptrs, nums, _p(loss), _s()), "sum_mean_squares_forward")
-        _lib.count(1)
+        _lib.call("mdb_sum_mean_squares_forward_f32", n, xs, nums, loss)
         ctx.save_for_backward(*xs)
         return loss
 
@@ -759,12 +725,8 @@ class _SumMeanSquares(Function):
         xs = ctx.saved_tensors
         n = len(xs)
         gs = [torch.empty_like(x) for x in xs]
-        ptrs = (_ct.c_void_p * n)(*[x.data_ptr() for x in xs])
-        gptrs = (_ct.c_void_p * n)(*[g.data_ptr() for g in gs])
         nums = (_ct.c_longlong * n)(*[x.numel() for x in xs])
-        dl = dloss.contiguous().float()
-        _lib.check(_lib.lib().mdb_sum_mean_squares_backward_f32(n, ptrs, gptrs, nums, _p(dl), _s()), "sum_mean_squares_backward")
-        _lib.count(1)
+        _lib.call("mdb_sum_mean_squares_backward_f32", n, xs, gs, nums, dloss.contiguous().float())
         return tuple(gs)
 
 

@@ -4,22 +4,6 @@ import torch
 from . import _lib
 
 
-def _s():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _p(t):
-    return 0 if t is None else t.data_ptr()
-
-
-def _chk(*ts):
-    for t in ts:
-        if t is None:
-            continue
-        if not t.is_cuda:
-            raise RuntimeError("monodetr_b200: CUDA tensors required (no CPU path)")
-
-
 # ---- dropout seed ------------------------------------------------------------------------------------------
 # Masks are a counter-based hash of (seed, site, element) -- csrc/rng.cuh -- so nothing but the seed is stored.  The seed
 # lives in device memory (a captured CUDA graph re-reads it at every replay).  There is one MASTER seed per device,
@@ -66,15 +50,9 @@ def seed_tensor(device):
     return snap if snap is not None else master_seed(device)
 
 
-def advance_seed(device):
-    """Kept for callers that drive the seed by hand: equivalent to begin_forward."""
-    begin_forward(device)
-
-
 # ---- attention ------------------------------------------------------------------------------------------
 def attention_forward(q, k, v, key_padding_mask=None, drop_p=0.0, site=0, seed=None):
     """q (B, Lq, H*32), k/v (B, Lk, H*32): last dim contiguous, token stride arbitrary (views of packed buffers ok)."""
-    _chk(q, k, v, key_padding_mask)
     B, Lq, E = q.shape
     Lk = k.shape[1]
     H = E // 32
@@ -86,10 +64,8 @@ def attention_forward(q, k, v, key_padding_mask=None, drop_p=0.0, site=0, seed=N
     if key_padding_mask is not None:
         kpm = key_padding_mask.to(torch.uint8).contiguous()
     seed = (seed if seed is not None else seed_tensor(q.device)) if drop_p > 0 else None
-    rc = _lib.lib().mdb_attention_forward_f32(_p(q), _p(k), _p(v), _p(kpm), _p(out), _p(lse), B, H, Lq, Lk, 32, q.stride(1),
-                                              k.stride(1), v.stride(1), E, float(drop_p), _p(seed), site, _s())
-    _lib.check(rc, "attention_forward")
-    _lib.count(1)
+    _lib.call("mdb_attention_forward_f32", q, k, v, kpm, out, lse, B, H, Lq, Lk, 32, q.stride(1), k.stride(1), v.stride(1), E,
+              float(drop_p), seed, site)
     return out, lse, kpm
 
 
@@ -103,17 +79,13 @@ def attention_backward(q, k, v, kpm, out, lse, dout, drop_p=0.0, site=0, seed=No
     dv = torch.empty((B, Lk, E), dtype=torch.float32, device=q.device)
     ws = torch.empty((B, H, Lq), dtype=torch.float32, device=q.device)
     seed = (seed if seed is not None else seed_tensor(q.device)) if drop_p > 0 else None
-    rc = _lib.lib().mdb_attention_backward_f32(_p(q), _p(k), _p(v), _p(kpm), _p(out), _p(lse), _p(dout), _p(ws), _p(dq), _p(dk),
-                                               _p(dv), B, H, Lq, Lk, 32, q.stride(1), k.stride(1), v.stride(1), E, E, E, E,
-                                               float(drop_p), _p(seed), site, _s())
-    _lib.check(rc, "attention_backward")
-    _lib.count(3)
+    _lib.call("mdb_attention_backward_f32", q, k, v, kpm, out, lse, dout, ws, dq, dk, dv, B, H, Lq, Lk, 32, q.stride(1),
+              k.stride(1), v.stride(1), E, E, E, E, float(drop_p), seed, site, launches=3)
     return dq, dk, dv
 
 
 # ---- layer norm ----------------------------------------------------------------------------------------
 def add_layernorm_forward(x, res, gamma, beta, eps=1e-5, drop_p=0.0, site=0, seed=None):
-    _chk(x, res, gamma, beta)
     C = x.shape[-1]
     M = x.numel() // C
     assert x.is_contiguous() and (res is None or (res.is_contiguous() and res.shape == x.shape))
@@ -121,10 +93,7 @@ def add_layernorm_forward(x, res, gamma, beta, eps=1e-5, drop_p=0.0, site=0, see
     mean = torch.empty((M,), dtype=torch.float32, device=x.device)
     rstd = torch.empty((M,), dtype=torch.float32, device=x.device)
     seed = (seed if seed is not None else seed_tensor(x.device)) if drop_p > 0 else None
-    rc = _lib.lib().mdb_add_layernorm_forward_f32(_p(x), _p(res), _p(gamma), _p(beta), _p(y), _p(mean), _p(rstd), M, C, eps,
-                                                  float(drop_p), _p(seed), site, _s())
-    _lib.check(rc, "add_layernorm_forward")
-    _lib.count(1)
+    _lib.call("mdb_add_layernorm_forward_f32", x, res, gamma, beta, y, mean, rstd, M, C, eps, float(drop_p), seed, site)
     return y, mean, rstd
 
 
@@ -137,17 +106,14 @@ def add_layernorm_backward(dy, x, res, gamma, mean, rstd, drop_p=0.0, site=0, se
     dgamma = torch.empty((C,), dtype=torch.float32, device=x.device)
     dbeta = torch.empty((C,), dtype=torch.float32, device=x.device)
     seed = (seed if seed is not None else seed_tensor(x.device)) if drop_p > 0 else None
-    rc = _lib.lib().mdb_add_layernorm_backward_f32(_p(dy), _p(x), _p(res), _p(gamma), _p(mean), _p(rstd), _p(dx), _p(dres),
-                                                   _p(dgamma), _p(dbeta), M, C, float(drop_p), _p(seed), site, 0, _s())
-    _lib.check(rc, "add_layernorm_backward")
-    _lib.count(1)
+    _lib.call("mdb_add_layernorm_backward_f32", dy, x, res, gamma, mean, rstd, dx, dres, dgamma, dbeta, M, C, float(drop_p), seed,
+              site, 0)
     return dx, (dres if dres is not None else dx), dgamma, dbeta
 
 
 # ---- group norm (NHWC) -----------------------------------------------------------------------------------
 def groupnorm_forward(x, gamma, beta, G=32, eps=1e-5, relu=False):
     """x (B, ..., C) channels-last contiguous."""
-    _chk(x, gamma, beta)
     assert x.is_contiguous()
     B, C = x.shape[0], x.shape[-1]
     HW = x.numel() // (B * C)
@@ -155,10 +121,7 @@ def groupnorm_forward(x, gamma, beta, G=32, eps=1e-5, relu=False):
     mean = torch.empty((B, G), dtype=torch.float32, device=x.device)
     rstd = torch.empty((B, G), dtype=torch.float32, device=x.device)
     ws = torch.empty((B, G, 2), dtype=torch.float64, device=x.device)
-    rc = _lib.lib().mdb_groupnorm_forward_f32(_p(x), _p(gamma), _p(beta), _p(y), _p(mean), _p(rstd), _p(ws), B, HW, C, G, eps,
-                                              int(relu), _s())
-    _lib.check(rc, "groupnorm_forward")
-    _lib.count(2)
+    _lib.call("mdb_groupnorm_forward_f32", x, gamma, beta, y, mean, rstd, ws, B, HW, C, G, eps, int(relu), launches=2)
     return y, mean, rstd
 
 
@@ -170,8 +133,6 @@ def groupnorm_backward(dy, x, y, gamma, mean, rstd, G=32, relu=False):
     dgamma = torch.empty((C,), dtype=torch.float32, device=x.device)
     dbeta = torch.empty((C,), dtype=torch.float32, device=x.device)
     ws = torch.empty((B, G, 2), dtype=torch.float64, device=x.device)
-    rc = _lib.lib().mdb_groupnorm_backward_f32(_p(dy), _p(x), _p(y if relu else None), _p(gamma), _p(mean), _p(rstd), _p(dx),
-                                               _p(dgamma), _p(dbeta), _p(ws), B, HW, C, G, int(relu), _s())
-    _lib.check(rc, "groupnorm_backward")
-    _lib.count(2)
+    _lib.call("mdb_groupnorm_backward_f32", dy, x, y if relu else None, gamma, mean, rstd, dx, dgamma, dbeta, ws, B, HW, C, G,
+              int(relu), launches=2)
     return dx, dgamma, dbeta

@@ -65,18 +65,15 @@ class FusedAdamW(torch.optim.Optimizer):
         lr, (beta1, beta2), eps = g0["lr"], g0["betas"], g0["eps"]
         wd = max(g["weight_decay"] for g in self.param_groups)
         self.step_count += 1
-        step_dev = 0
+        step_dev = None
         if self.device_step:                          # graph-safe: t and the bias corrections live on the device
             self._t += 1
             self._step_size.copy_(lr * torch.sqrt(1 - beta2 ** self._t) / (1 - beta1 ** self._t))
-            step_size, step_dev = 0.0, self._step_size.data_ptr()
+            step_size, step_dev = 0.0, self._step_size
         else:
             step_size = lr * math.sqrt(1 - beta2 ** self.step_count) / (1 - beta1 ** self.step_count)
-        rc = _lib.lib().mdb_adamw_step_f32(self.flat_p.data_ptr(), b.flat.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                                           b.numel, b.n_decay, beta1, 1 - beta1, beta2, 1 - beta2, eps, wd, step_size, step_dev,
-                                           torch.cuda.current_stream().cuda_stream)
-        _lib.check(rc, "adamw_step")
-        _lib.count(1)
+        _lib.call("mdb_adamw_step_f32", self.flat_p, b.flat, self.exp_avg, self.exp_avg_sq, b.numel, b.n_decay, beta1, 1 - beta1, beta2,
+                  1 - beta2, eps, wd, step_size, step_dev)
         return loss
 
     def zero_grad(self, set_to_none=True):

@@ -96,8 +96,6 @@ class ImageBatchPreprocessor:
         W, H = self.resolution
         out = torch.empty(B, 3, H, W, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().mdb_warp_affine_normalize_u8(ptrs, whd, pitch, trd, fld, B,
-                                                               W, H, self.mean.ctypes.data, self.std.ctypes.data, out.data_ptr(),
-                                                               torch.cuda.current_stream().cuda_stream), "warp_affine_normalize")
-        _lib.count(1)
+            _lib.call("mdb_warp_affine_normalize_u8", ptrs, whd, pitch, trd, fld, B, W, H, self.mean.ctypes.data, self.std.ctypes.data,
+                      out)
         return out

@@ -9,20 +9,10 @@ import torch
 from . import _lib
 
 
-def _s():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _p(t):
-    return 0 if t is None else t.data_ptr()
-
-
 def _chk(*ts):
     for t in ts:
         if t is None:
             continue
-        if not t.is_cuda:
-            raise RuntimeError("monodetr_b200.tc: CUDA tensors required (no CPU path)")
         if t.dtype != torch.float32 or not t.is_contiguous():
             raise RuntimeError("monodetr_b200.tc: contiguous float32 tensors required")
 
@@ -36,13 +26,8 @@ def pack_weight(w_oihw, scale=None):
     _chk(w_oihw, scale)
     O, I, kh, kw = w_oihw.shape
     out = torch.empty((kh * kw, O, I), dtype=torch.float32, device=w_oihw.device)
-    _lib.check(_lib.lib().mdb_pack_conv_weight_f32(_p(w_oihw), _p(scale), _p(out), O, I, kh * kw, _s()), "pack_weight")
-    _lib.count(1)
+    _lib.call("mdb_pack_conv_weight_f32", w_oihw, scale, out, O, I, kh * kw)
     return out
-
-
-def _ptr_array(tensors):
-    return (ctypes.c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
 
 
 def _int_array(vals):
@@ -92,11 +77,8 @@ def split_weights(weights, scales=None, need_dgrad=True, packed_src=False):
         outs.append(SplitW(wf, wd, t, O, I))
         wfs.append(wf)
         wds.append(wd)
-    rc = _lib.lib().mdb_pack_gemm_weights_bf16x3(
-        n, _ptr_array(weights), _ptr_array(scales), _ptr_array(wfs), _ptr_array(wds), _int_array([d[1] for d in dims]),
-        _int_array([d[2] for d in dims]), _int_array([d[0] for d in dims]), int(packed_src), _s())
-    _lib.check(rc, "pack_gemm_weights_bf16x3")
-    _lib.count((n + 63) // 64)
+    _lib.call("mdb_pack_gemm_weights_bf16x3", n, weights, scales, wfs, wds, _int_array([d[1] for d in dims]),
+              _int_array([d[2] for d in dims]), _int_array([d[0] for d in dims]), int(packed_src), launches=(n + 63) // 64)
     return outs
 
 
@@ -165,11 +147,9 @@ def pack_weights_multi(weights, scales=None):
         O, I, kh, kw = w.shape
         outs.append(flat[off:off + sz].view(kh * kw, O, I))
         off += sz
-    rc = _lib.lib().mdb_pack_conv_weights_multi_f32(
-        n, _ptr_array(weights), _ptr_array(scales), _ptr_array(outs), _int_array([w.shape[0] for w in weights]),
-        _int_array([w.shape[1] for w in weights]), _int_array([w.shape[2] * w.shape[3] for w in weights]), _s())
-    _lib.check(rc, "pack_weights_multi")
-    _lib.count((n + 63) // 64)
+    _lib.call("mdb_pack_conv_weights_multi_f32", n, weights, scales, outs, _int_array([w.shape[0] for w in weights]),
+              _int_array([w.shape[1] for w in weights]), _int_array([w.shape[2] * w.shape[3] for w in weights]),
+              launches=(n + 63) // 64)
     return outs
 
 
@@ -181,11 +161,9 @@ def unpack_wgrads_multi(dw_packed_list, khw_list):
     _chk(*dw_packed_list)
     outs = [torch.empty((d.shape[1], d.shape[2], kh, kw), dtype=torch.float32, device=d.device)
             for d, (kh, kw) in zip(dw_packed_list, khw_list)]
-    rc = _lib.lib().mdb_unpack_conv_wgrads_multi_f32(
-        n, _ptr_array(dw_packed_list), _ptr_array(outs), _int_array([d.shape[1] for d in dw_packed_list]),
-        _int_array([d.shape[2] for d in dw_packed_list]), _int_array([d.shape[0] for d in dw_packed_list]), _s())
-    _lib.check(rc, "unpack_wgrads_multi")
-    _lib.count((n + 63) // 64)
+    _lib.call("mdb_unpack_conv_wgrads_multi_f32", n, dw_packed_list, outs, _int_array([d.shape[1] for d in dw_packed_list]),
+              _int_array([d.shape[2] for d in dw_packed_list]), _int_array([d.shape[0] for d in dw_packed_list]),
+              launches=(n + 63) // 64)
     return outs
 
 
@@ -193,8 +171,7 @@ def unpack_wgrad(dw_packed, kh, kw):
     _chk(dw_packed)
     taps, O, I = dw_packed.shape
     out = torch.empty((O, I, kh, kw), dtype=torch.float32, device=dw_packed.device)
-    _lib.check(_lib.lib().mdb_unpack_conv_wgrad_f32(_p(dw_packed), _p(out), O, I, taps, 0, _s()), "unpack_wgrad")
-    _lib.count(1)
+    _lib.call("mdb_unpack_conv_wgrad_f32", dw_packed, out, O, I, taps, 0)
     return out
 
 
@@ -202,8 +179,7 @@ def colsum(x2d):
     _chk(x2d)
     M, N = x2d.shape
     out = torch.empty((N,), dtype=torch.float32, device=x2d.device)
-    _lib.check(_lib.lib().mdb_colsum_f32(_p(x2d), _p(out), M, N, 0, _s()), "colsum")
-    _lib.count(1)
+    _lib.call("mdb_colsum_f32", x2d, out, M, N, 0)
     return out
 
 
@@ -227,20 +203,14 @@ def conv2d_forward(x, w_packed, bias=None, residual=None, kh=1, kw=1, stride=1, 
     if residual is not None:
         assert residual.shape == y.shape
     flags = int(relu) | (int(round_out) << 1)
-    L = _lib.lib()
-    need = L.mdb_conv2d_forward_workspace_bytes(B, H, W, Cin, Cout, kh, kw, stride, pad, flags, int(residual is not None), int(split))
+    need = _lib.lib().mdb_conv2d_forward_workspace_bytes(B, H, W, Cin, Cout, kh, kw, stride, pad, flags, int(residual is not None),
+                                                         int(split))
     if need < 0:
         _lib.check(int(need), "conv2d_forward_workspace_bytes")
     if need > 0:
         _ensure_workspace(x.device, need)
-    if split:
-        rc = L.mdb_conv2d_forward_bf16x3(_p(x), _p(w_packed.wf), _p(bias), _p(residual), _p(y), B, H, W, Cin, Cout, kh, kw,
-                                         stride, pad, flags, _s())
-    else:
-        rc = L.mdb_conv2d_forward_f32(_p(x), _p(w_packed), _p(bias), _p(residual), _p(y), B, H, W, Cin, Cout, kh, kw,
-                                      stride, pad, flags, _s())
-    _lib.check(rc, "conv2d_forward")
-    _lib.count(2 if need > 0 else 1)
+    _lib.call("mdb_conv2d_forward_bf16x3" if split else "mdb_conv2d_forward_f32", x, w_packed.wf if split else w_packed, bias,
+              residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, flags, launches=2 if need > 0 else 1)
     return y
 
 
@@ -259,14 +229,8 @@ def conv2d_dgrad(dy, w_packed, x_shape, residual=None, relu_mask=None, kh=1, kw=
     else:
         assert dy.shape[-1] == Cout
     dx = torch.empty((B, H, W, Cin), dtype=torch.float32, device=dy.device)
-    if split:
-        rc = _lib.lib().mdb_conv2d_dgrad_bf16x3(_p(dy), _p(w_packed.wd), _p(residual), _p(relu_mask), _p(dx), B, H, W, Cin,
-                                                Cout, kh, kw, stride, pad, int(round_out) << 1, _s())
-    else:
-        rc = _lib.lib().mdb_conv2d_dgrad_f32(_p(dy), _p(w_packed), _p(residual), _p(relu_mask), _p(dx), B, H, W, Cin, Cout, kh,
-                                             kw, stride, pad, int(round_out) << 1, _s())
-    _lib.check(rc, "conv2d_dgrad")
-    _lib.count(stride * stride)
+    _lib.call("mdb_conv2d_dgrad_bf16x3" if split else "mdb_conv2d_dgrad_f32", dy, w_packed.wd if split else w_packed, residual,
+              relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, int(round_out) << 1, launches=stride * stride)
     return dx
 
 
@@ -280,10 +244,8 @@ def conv2d_wgrad(dy, x, rowscale=None, kh=1, kw=1, stride=1, pad=0, with_bias_gr
     buf = torch.empty((n + (Cout if with_bias_grad else 0),), dtype=torch.float32, device=x.device)
     dwp = buf[:n].view(kh * kw, Cout, Cin)
     db = buf[n:] if with_bias_grad else None
-    rc = _lib.lib().mdb_conv2d_wgrad_bias_f32(_p(dy), _p(x), _p(rowscale), _p(dwp), _p(db), B, H, W, Cin, Cout, kh, kw, stride,
-                                              pad, 0, _s())
-    _lib.check(rc, "conv2d_wgrad")
-    _lib.count(1 if (not with_bias_grad or get_precision() != "tf32") else 2)
+    _lib.call("mdb_conv2d_wgrad_bias_f32", dy, x, rowscale, dwp, db, B, H, W, Cin, Cout, kh, kw, stride, pad, 0,
+              launches=1 if (not with_bias_grad or get_precision() != "tf32") else 2)
     return (dwp, db) if with_bias_grad else dwp
 
 
@@ -305,8 +267,7 @@ def round_tf32(x):
     if _lib.lib().mdb_get_precision() != 0:
         return x
     out = torch.empty_like(x)
-    _lib.check(_lib.lib().mdb_round_tf32_f32(_p(x), _p(out), x.numel(), _s()), "round_tf32")
-    _lib.count(1)
+    _lib.call("mdb_round_tf32_f32", x, out, x.numel())
     return out
 
 

@@ -43,6 +43,23 @@ def test_cpu_tensor_is_rejected_loudly():
         ms_deform_attn_forward(v, sh, ls, loc, at, 64)
 
 
+def test_cpu_tensor_is_rejected_by_every_wrapper():
+    """Host tensors never reach a launch: the library call names its entry point and raises before any CUDA call."""
+    import pytest
+    import torch
+    from monodetr_b200 import functional as Fn
+    n0 = _lib.launch_count()
+    with pytest.raises(RuntimeError, match="mdb_box_refine_forward_f32: CUDA tensors required"):
+        Fn.box_refine(torch.zeros(2, 6), torch.full((2, 2), 0.5))
+    with pytest.raises(RuntimeError, match="mdb_mean3_f32: CUDA tensors required"):
+        Fn.mean3(torch.zeros(8), torch.zeros(8), torch.zeros(8))
+    with pytest.raises(RuntimeError, match="mdb_depth_sample_forward_f32: CUDA tensors required"):
+        Fn.depth_sample(torch.zeros(1, 4, 4), torch.zeros(1, 3, 2))
+    with pytest.raises(RuntimeError, match="mdb_sum_mean_squares_forward_f32: CUDA tensors required"):
+        Fn.sum_mean_squares([torch.zeros(4), torch.zeros(8)])          # tensors inside a pointer array are checked too
+    assert _lib.launch_count() == n0
+
+
 def test_process_wide_settings_round_trip_without_a_gpu():
     """mdb_set_deterministic / mdb_set_precision are host-side switches: they answer on a machine without a GPU."""
     import monodetr_b200

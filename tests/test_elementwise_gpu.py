@@ -33,14 +33,12 @@ def test_stem_conv_bn_relu_and_maxpool(B, H, W):
         shift = torch.randn(64, device="cuda", generator=g)
         H1, W1 = (H + 6 - 7) // 2 + 1, (W + 6 - 7) // 2 + 1
         y = torch.empty(B, H1, W1, 64, device="cuda")
-        s = torch.cuda.current_stream().cuda_stream
-        _lib.check(_lib.lib().mdb_stem_conv7x7_bn_relu_f32(x.data_ptr(), w.data_ptr(), scale.data_ptr(), shift.data_ptr(),
-                                                           y.data_ptr(), B, H, W, s), "stem")
+        _lib.call("mdb_stem_conv7x7_bn_relu_f32", x, w, scale, shift, y, B, H, W)
         ref = torch.relu(F.conv2d(x, w, None, stride=2, padding=3) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
         assert _rel(y.permute(0, 3, 1, 2), ref) < 1e-5          # plain fp32 CUDA-core kernel
         H2, W2 = (H1 + 2 - 3) // 2 + 1, (W1 + 2 - 3) // 2 + 1
         p = torch.empty(B, H2, W2, 64, device="cuda")
-        _lib.check(_lib.lib().mdb_maxpool3x3s2_nhwc_f32(y.data_ptr(), p.data_ptr(), B, H1, W1, 64, s), "maxpool")
+        _lib.call("mdb_maxpool3x3s2_nhwc_f32", y, p, B, H1, W1, 64)
         assert torch.equal(p.permute(0, 3, 1, 2), F.max_pool2d(y.permute(0, 3, 1, 2), 3, 2, 1))   # exact: a selection
     finally:
         tc.set_precision(prev)
