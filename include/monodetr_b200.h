@@ -32,15 +32,23 @@ int mdb_abi_version(void);
 /* Human-readable name of the last error code returned on this thread ("ok" if 0). HOST string. */
 const char* mdb_error_string(int code);
 
-/* Reproducible accumulation (process-wide; default 0).  The reference scatters the MSDeformAttn value gradient with atomicAdd
- * (ms_deform_im2col_cuda.cuh:125-152) and so does the default path here (vector reductions), as does the split-K weight gradient
- * of the tensor-core family: results then differ in the last bits from run to run.  With 1:
- *   - mdb_msda_backward_f32 / _f64 accumulate grad_value in a FIXED order (one thread owns each element and adds its
- *     contributions in (query, point, corner) order with plain read-modify-writes; grad_loc / grad_attn never use atomics),
- *   - mdb_msda_fused_backward_f32 returns MDB_EUNSUPPORTED (callers take mdb_msda_prep_* + mdb_msda_backward_*),
- *   - mdb_conv2d_wgrad_* run without split-K (exactly one accumulation per output element),
- * so that two runs on the same inputs give the same bits.  A test / debugging mode: the ordered scatter walks every query serially per (image, head, level): 32 ms instead of 0.95 ms at B = 8, Lq = 10 200.
- * (Per-channel parameter gradients of the norm layers and the GroupNorm statistics still combine CTA partials atomically.) */
+/* Reproducible mode (process-wide; default 0).  By default the MSDeformAttn value gradient (like the reference's kernel,
+ * ms_deform_im2col_cuda.cuh:125-152), the split-K weight gradients, the norm-parameter gradients, the GroupNorm statistics, the
+ * depth-map gradients of the heads and the depth tail's embedding gradient combine partial sums with float atomics, so results
+ * differ in the last bits from run to run.  With 1, every floating-point output element has exactly one writer that adds its terms
+ * in an order fixed by the problem shape (never by the SM count or the scheduling):
+ *   - mdb_msda_backward_f32 / _f64 accumulate grad_value in (query, point, corner) order; mdb_msda_fused_backward_f32 returns
+ *     MDB_EUNSUPPORTED (callers take mdb_msda_prep_* + mdb_msda_backward_*),
+ *   - mdb_conv2d_wgrad_* run without split-K and mdb_colsum_f32 in one pass,
+ *   - mdb_add_layernorm_backward_f32: dgamma / dbeta in a second launch (fixed row partition, combined in a thread-block cluster),
+ *   - mdb_groupnorm_forward_f32 / _backward_f32: one CTA per (group, image) / per group writes the statistics and dgamma / dbeta,
+ *   - mdb_head_depth_backward_f32 / mdb_depth_sample_backward_f32: the map gradient in gather form (a second launch for the former),
+ *   - mdb_depth_tail_backward_f32: demb in a second launch, per (row, channel) over the pixels in pixel order,
+ *   - mdb_sum_mean_squares_forward_f32 reduces in one CTA in tensor order.
+ * Integer atomics (criterion counts, decode count) are exact and stay.  Guarantee: on the same GPU model with the same build, in
+ * one process, two runs of a training iteration (forward with dropout, the device criterion, backward, mdb_adamw_step_f32) from
+ * the same weights, optimizer state, inputs and dropout seed give identical bits, eagerly or as a replayed CUDA graph.  Not
+ * covered: the reduction order of a multi-GPU all-reduce.  A test / debugging mode, several times slower (DESIGN.md section 5). */
 int mdb_set_deterministic(int on);
 int mdb_get_deterministic(void);
 
@@ -242,6 +250,11 @@ int mdb_depth_tail_forward_f32(const float* logits, const float* bins, const flo
                                int E, int C, float dmax, void* stream);
 int mdb_depth_tail_backward_f32(const float* logits, const float* bins, const float* emb, const float* d_ip, const float* d_wd_ext,
                                 float* dlogits, float* demb, long long npix, int nb, int E, int C, float dmax, void* stream);
+/* F.interpolate(mode="bilinear", align_corners=False) to a given size on NHWC maps: x (B,Hi,Wi,C) -> y (B,Ho,Wo,C), C % 4 == 0.
+ * src = (in / out) * (dst + 0.5) - 0.5 clamped at 0, i1 = i0 + (i0 < in - 1) (torch's rule).  backward: dx (B,Hi,Wi,C) fully
+ * written in gather form (no atomics, bit-reproducible). */
+int mdb_upsample_bilinear_nhwc_forward_f32(const float* x, float* y, int B, int Hi, int Wi, int Ho, int Wo, int C, void* stream);
+int mdb_upsample_bilinear_nhwc_backward_f32(const float* dy, float* dx, int B, int Hi, int Wi, int Ho, int Wo, int C, void* stream);
 /* (a + b + c) / 3 and a * s; n % 4 == 0 */
 int mdb_mean3_f32(const float* a, const float* b, const float* c, float* out, long long n, void* stream);
 int mdb_scale_f32(const float* a, float* out, long long n, float s, void* stream);

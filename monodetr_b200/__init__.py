@@ -11,10 +11,13 @@ def build_monodetr(cfg, criterion_builder=None):
 
 
 def set_deterministic(on=True):
-    """Reproducible accumulation for the two large scatter sites (`mdb_set_deterministic`, include/monodetr_b200.h): the
-    MSDeformAttn value gradient is accumulated in a fixed order (the reference's kernel and the default path here scatter
-    with atomics, ms_deform_im2col_cuda.cuh:125-152) and weight gradients run without split-K.  A test / debugging mode
-    (much slower); set it before the forward pass.  Returns the previous setting."""
+    """Reproducible mode (`mdb_set_deterministic`, include/monodetr_b200.h): every float accumulation of the training iteration
+    runs in a fixed order (the default path, like the reference's kernel, combines partial sums with atomics), and the depth
+    predictor resizes with the library's kernel instead of F.interpolate.  On the same GPU model and build, in one process, with
+    the device criterion, two training iterations from the same weights, optimizer state, inputs, targets and dropout seed
+    (torch.manual_seed, or kernels.reseed) give identical bits, eagerly or as a replayed CUDA graph; multi-GPU all-reduce order
+    is not covered.  A test / debugging mode: 4.4x slower per training step on an H100 (DESIGN.md section 5).  Set it before the
+    model is built.  Returns the previous setting."""
     from . import _lib
     prev = bool(_lib.lib().mdb_get_deterministic())
     _lib.check(_lib.lib().mdb_set_deterministic(1 if on else 0), "set_deterministic")

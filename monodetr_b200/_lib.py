@@ -63,6 +63,8 @@ SIGNATURES = {
     "mdb_head_depth_backward_f32": [_PTR] * 10 + [c_int] * 4 + [_PTR],
     "mdb_depth_tail_forward_f32": [_PTR] * 5 + [ctypes.c_longlong, c_int, c_int, c_int, c_float, _PTR],
     "mdb_depth_tail_backward_f32": [_PTR] * 7 + [ctypes.c_longlong, c_int, c_int, c_int, c_float, _PTR],
+    "mdb_upsample_bilinear_nhwc_forward_f32": [_PTR] * 2 + [c_int] * 6 + [_PTR],
+    "mdb_upsample_bilinear_nhwc_backward_f32": [_PTR] * 2 + [c_int] * 6 + [_PTR],
     "mdb_mean3_f32": [_PTR] * 4 + [ctypes.c_longlong, _PTR],
     "mdb_scale_f32": [_PTR] * 2 + [ctypes.c_longlong, c_float, _PTR],
     "mdb_sum_mean_squares_forward_f32": [c_int, _PTR, _PTR, _PTR, _PTR],
@@ -93,6 +95,10 @@ def lib():
             fn.argtypes = argtypes
             fn.restype = _RESTYPES.get(name, c_int)
         _lib = L
+        # MDB_DETERMINISTIC=1: the process starts in reproducible mode (mdb_set_deterministic), so that a program that never calls
+        # set_deterministic -- bench.py, a training script -- can be run twice and compared bit for bit; set_deterministic overrides it
+        if os.environ.get("MDB_DETERMINISTIC") == "1":
+            check(L.mdb_set_deterministic(1), "mdb_set_deterministic")
     return _lib
 
 
@@ -129,6 +135,12 @@ def call(name: str, *args, launches: int = 1):
         conv.append(a)
     check(getattr(lib(), name)(*conv, torch.cuda.current_stream().cuda_stream), name)
     count(launches)
+
+
+def deterministic() -> bool:
+    """Whether the library is in reproducible mode (mdb_set_deterministic); some entry points then launch a different number of
+    kernels."""
+    return bool(lib().mdb_get_deterministic())
 
 
 def count(n: int = 1):

@@ -533,6 +533,111 @@ __global__ void depth_sample_bwd_kernel(const float* __restrict__ dout, const fl
     put(y0, x0, (1.f - ly) * (1.f - lx)); put(y0, x0 + 1, (1.f - ly) * lx); put(y0 + 1, x0, ly * (1.f - lx)); put(y0 + 1, x0 + 1, ly * lx);
 }
 
+// Reproducible mode: the map gradient in gather form -- one thread per map pixel walks the N centres of its image in order.
+__global__ void depth_sample_bwd_gather_kernel(const float* __restrict__ dout, const float* __restrict__ xy, float* __restrict__ ddepth,
+                                               int B, int H, int W, int N) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * H * W) return;
+    const int b = i / (H * W), py = (i / W) % H, px = i % W;
+    float acc = 0.f;
+    for (int q = b * N; q < (b + 1) * N; ++q) {
+        const float x = (xy[2 * q] + 1.f) * 0.5f * (float)(W - 1), y = (xy[2 * q + 1] + 1.f) * 0.5f * (float)(H - 1);
+        const float xf = floorf(x), yf = floorf(y);
+        const int x0 = (int)xf, y0 = (int)yf;
+        if ((y0 != py && y0 + 1 != py) || (x0 != px && x0 + 1 != px)) continue;
+        const float lx = x - xf, ly = y - yf, g = dout[q];
+        if (y0 == py && x0 == px) acc += ((1.f - ly) * (1.f - lx)) * g;
+        if (y0 == py && x0 + 1 == px) acc += ((1.f - ly) * lx) * g;
+        if (y0 + 1 == py && x0 == px) acc += (ly * (1.f - lx)) * g;
+        if (y0 + 1 == py && x0 + 1 == px) acc += (ly * lx) * g;
+    }
+    ddepth[i] = acc;
+}
+
+// ---- bilinear resize of NHWC maps, F.interpolate(mode="bilinear", align_corners=False) without a scale factor ------------
+// torch's source-index rule: src = (in / out) * (dst + 0.5) - 0.5, clamped below at 0; i0 = floor(src), i1 = i0 + (i0 < in - 1),
+// lambda1 = src - i0, lambda0 = 1 - lambda1.
+__device__ __forceinline__ void up_src(int o, float scale, int in, int& i0, int& i1, float& l0, float& l1) {
+    float s = scale * ((float)o + 0.5f) - 0.5f;
+    if (s < 0.f) s = 0.f;
+    i0 = (int)s;
+    i1 = i0 + (i0 < in - 1 ? 1 : 0);
+    l1 = s - (float)i0;
+    l0 = 1.f - l1;
+}
+
+// one thread per (b, oy, ox, channel quad)
+__global__ void upsample_bilinear_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int Hi, int Wi, int Ho, int Wo,
+                                             int C, float sh, float sw) {
+    const int c4n = C / 4;
+    const long long n4 = (long long)B * Ho * Wo * c4n;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i % c4n) * 4;
+        long long r = i / c4n;
+        const int ox = (int)(r % Wo); r /= Wo;
+        const int oy = (int)(r % Ho);
+        const int b = (int)(r / Ho);
+        int h0, h1, w0, w1; float hl0, hl1, wl0, wl1;
+        up_src(oy, sh, Hi, h0, h1, hl0, hl1);
+        up_src(ox, sw, Wi, w0, w1, wl0, wl1);
+        const float* xb = x + (size_t)b * Hi * Wi * C + c;
+        const float4 a = *reinterpret_cast<const float4*>(xb + ((size_t)h0 * Wi + w0) * C);
+        const float4 bb = *reinterpret_cast<const float4*>(xb + ((size_t)h0 * Wi + w1) * C);
+        const float4 cc = *reinterpret_cast<const float4*>(xb + ((size_t)h1 * Wi + w0) * C);
+        const float4 d = *reinterpret_cast<const float4*>(xb + ((size_t)h1 * Wi + w1) * C);
+        float4 o;
+        o.x = hl0 * (wl0 * a.x + wl1 * bb.x) + hl1 * (wl0 * cc.x + wl1 * d.x);
+        o.y = hl0 * (wl0 * a.y + wl1 * bb.y) + hl1 * (wl0 * cc.y + wl1 * d.y);
+        o.z = hl0 * (wl0 * a.z + wl1 * bb.z) + hl1 * (wl0 * cc.z + wl1 * d.z);
+        o.w = hl0 * (wl0 * a.w + wl1 * bb.w) + hl1 * (wl0 * cc.w + wl1 * d.w);
+        *reinterpret_cast<float4*>(y + i * 4) = o;
+    }
+}
+
+// Gather form of the backward (deterministic by construction): one thread per (b, h, w, channel quad) of the input walks the output
+// rows / columns whose source window can contain it, in increasing order, and adds lambda_h * lambda_w * dy for each corner that is it.
+__global__ void upsample_bilinear_bwd_kernel(const float* __restrict__ dy, float* __restrict__ dx, int B, int Hi, int Wi, int Ho, int Wo,
+                                             int C, float sh, float sw) {
+    const int c4n = C / 4;
+    const long long n4 = (long long)B * Hi * Wi * c4n;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i % c4n) * 4;
+        long long r = i / c4n;
+        const int w = (int)(r % Wi); r /= Wi;
+        const int h = (int)(r % Hi);
+        const int b = (int)(r / Hi);
+        // outputs with src in [h - 1, h + 1): (dst + 0.5) * scale in [h - 0.5, h + 1.5), widened by 2 against rounding; the rows whose
+        // src is clamped to 0 start at dst 0
+        const int ylo = h <= 1 ? 0 : max(0, (int)floorf((h - 0.5f) / sh - 0.5f) - 2);
+        const int yhi = min(Ho - 1, (int)ceilf((h + 1.5f) / sh - 0.5f) + 2);
+        const int xlo = w <= 1 ? 0 : max(0, (int)floorf((w - 0.5f) / sw - 0.5f) - 2);
+        const int xhi = min(Wo - 1, (int)ceilf((w + 1.5f) / sw - 0.5f) + 2);
+        const float* gb = dy + (size_t)b * Ho * Wo * C + c;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int oy = ylo; oy <= yhi; ++oy) {
+            int h0, h1; float hl0, hl1;
+            up_src(oy, sh, Hi, h0, h1, hl0, hl1);
+            if (h0 != h && h1 != h) continue;
+            for (int ox = xlo; ox <= xhi; ++ox) {
+                int w0, w1; float wl0, wl1;
+                up_src(ox, sw, Wi, w0, w1, wl0, wl1);
+                if (w0 != w && w1 != w) continue;
+                const float4 g = *reinterpret_cast<const float4*>(gb + ((size_t)oy * Wo + ox) * C);
+                float f[4] = {0.f, 0.f, 0.f, 0.f};
+                int k = 0;
+                if (h0 == h && w0 == w) f[k++] = hl0 * wl0;
+                if (h0 == h && w1 == w) f[k++] = hl0 * wl1;
+                if (h1 == h && w0 == w) f[k++] = hl1 * wl0;
+                if (h1 == h && w1 == w) f[k++] = hl1 * wl1;
+                for (int j = 0; j < k; ++j) {
+                    acc.x += f[j] * g.x; acc.y += f[j] * g.y; acc.z += f[j] * g.z; acc.w += f[j] * g.w;
+                }
+            }
+        }
+        *reinterpret_cast<float4*>(dx + i * 4) = acc;
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -548,10 +653,31 @@ int mdb_depth_sample_forward_f32(const float* depth, const float* xy, float* out
 int mdb_depth_sample_backward_f32(const float* dout, const float* xy, float* ddepth, int B, int H, int W, int N, void* stream_) {
     if (!dout || !xy || !ddepth || B <= 0 || H <= 0 || W <= 0 || N < 0) return MDB_EINVAL;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (mdb_get_deterministic()) {                   // reproducible mode: gather, every pixel written once
+        depth_sample_bwd_gather_kernel<<<(B * H * W + 127) / 128, 128, 0, stream>>>(dout, xy, ddepth, B, H, W, N);
+        return (int)cudaGetLastError();
+    }
     cudaError_t e = cudaMemsetAsync(ddepth, 0, sizeof(float) * (size_t)B * H * W, stream);
     if (e != cudaSuccess) return (int)e;
     if (N == 0) return 0;
     depth_sample_bwd_kernel<<<(B * N + 127) / 128, 128, 0, stream>>>(dout, xy, ddepth, B, H, W, N);
+    return (int)cudaGetLastError();
+}
+
+// x (B, Hi, Wi, C) -> y (B, Ho, Wo, C), NHWC contiguous, C % 4 == 0, 16-byte aligned.
+int mdb_upsample_bilinear_nhwc_forward_f32(const float* x, float* y, int B, int Hi, int Wi, int Ho, int Wo, int C, void* stream) {
+    if (!x || !y || B <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || C <= 0 || C % 4) return MDB_EINVAL;
+    const long long n4 = (long long)B * Ho * Wo * C / 4;
+    upsample_bilinear_fwd_kernel<<<grid_cap(n4, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        x, y, B, Hi, Wi, Ho, Wo, C, (float)Hi / (float)Ho, (float)Wi / (float)Wo);
+    return (int)cudaGetLastError();
+}
+// dx (B, Hi, Wi, C) = gradient wrt x of the forward above for dy (B, Ho, Wo, C); fully written, no atomics.
+int mdb_upsample_bilinear_nhwc_backward_f32(const float* dy, float* dx, int B, int Hi, int Wi, int Ho, int Wo, int C, void* stream) {
+    if (!dy || !dx || B <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || C <= 0 || C % 4) return MDB_EINVAL;
+    const long long n4 = (long long)B * Hi * Wi * C / 4;
+    upsample_bilinear_bwd_kernel<<<grid_cap(n4, 256, num_sms() * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        dy, dx, B, Hi, Wi, Ho, Wo, C, (float)Hi / (float)Ho, (float)Wi / (float)Wo);
     return (int)cudaGetLastError();
 }
 

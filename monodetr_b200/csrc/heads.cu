@@ -11,10 +11,14 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <cooperative_groups.h>
+
 #include "../../include/monodetr_b200.h"
 #include "launch.cuh"
 
 namespace {
+
+namespace cg = cooperative_groups;
 
 using namespace mdb;
 
@@ -81,7 +85,9 @@ __global__ void head_depth_fwd_kernel(const float* __restrict__ coord, const flo
     out[2 * i] = (dr + geo + dm) / 3.f;
     out[2 * i + 1] = reg[2 * i + 1];
 }
-// dwdepth must be zero-filled (or hold other contributions): accumulated with atomics
+// dwdepth must be zero-filled (or hold other contributions): accumulated with atomics.  SCATTER = false (reproducible mode):
+// the map gradient is left to head_depth_bwd_gather_kernel.
+template <bool SCATTER = true>
 __global__ void head_depth_bwd_kernel(const float* __restrict__ dout, const float* __restrict__ coord, const float* __restrict__ size3d,
                                       const float* __restrict__ reg, const float* __restrict__ calibs, const float* __restrict__ img_sizes,
                                       float* __restrict__ dcoord, float* __restrict__ dsize3d, float* __restrict__ dreg,
@@ -107,11 +113,35 @@ __global__ void head_depth_bwd_kernel(const float* __restrict__ dout, const floa
     const float den = sg + 1e-6f;
     dreg[2 * i] = -g * sg * (1.f - sg) / (den * den);
     dreg[2 * i + 1] = dout[2 * i + 1];
-    int x0, y0; float lx, ly;
-    bilinear_ac((c[0] - 0.5f) * 2.f, (c[1] - 0.5f) * 2.f, H, W, x0, y0, lx, ly);
-    float* d = dwdepth + (size_t)b * H * W;
-    auto put = [&](int yy, int xx, float w) { if (xx >= 0 && xx <= W - 1 && yy >= 0 && yy <= H - 1) atomicAdd(d + yy * W + xx, w * g); };
-    put(y0, x0, (1.f - ly) * (1.f - lx)); put(y0, x0 + 1, (1.f - ly) * lx); put(y0 + 1, x0, ly * (1.f - lx)); put(y0 + 1, x0 + 1, ly * lx);
+    if constexpr (SCATTER) {
+        int x0, y0; float lx, ly;
+        bilinear_ac((c[0] - 0.5f) * 2.f, (c[1] - 0.5f) * 2.f, H, W, x0, y0, lx, ly);
+        float* d = dwdepth + (size_t)b * H * W;
+        auto put = [&](int yy, int xx, float w) { if (xx >= 0 && xx <= W - 1 && yy >= 0 && yy <= H - 1) atomicAdd(d + yy * W + xx, w * g); };
+        put(y0, x0, (1.f - ly) * (1.f - lx)); put(y0, x0 + 1, (1.f - ly) * lx); put(y0 + 1, x0, ly * (1.f - lx)); put(y0 + 1, x0 + 1, ly * lx);
+    }
+}
+// Reproducible mode: the same map gradient in gather form.  One thread per map pixel walks the queries of its image in index order
+// and adds the corner weight of every query that samples it (same arithmetic as the scatter above); every pixel is written.
+__global__ void head_depth_bwd_gather_kernel(const float* __restrict__ dout, const float* __restrict__ coord, float* __restrict__ dwdepth,
+                                             int B, int N, int H, int W) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * H * W) return;
+    const int b = i / (H * W), py = (i / W) % H, px = i % W;
+    float acc = 0.f;
+    for (int q = b * N; q < (b + 1) * N; ++q) {
+        const float* c = coord + (size_t)q * 6;
+        int x0, y0; float lx, ly;
+        bilinear_ac((c[0] - 0.5f) * 2.f, (c[1] - 0.5f) * 2.f, H, W, x0, y0, lx, ly);
+        if (y0 != py && y0 + 1 != py) continue;
+        if (x0 != px && x0 + 1 != px) continue;
+        const float g = dout[2 * q] / 3.f;
+        if (y0 == py && x0 == px) acc += ((1.f - ly) * (1.f - lx)) * g;
+        if (y0 == py && x0 + 1 == px) acc += ((1.f - ly) * lx) * g;
+        if (y0 + 1 == py && x0 == px) acc += (ly * (1.f - lx)) * g;
+        if (y0 + 1 == py && x0 + 1 == px) acc += (ly * lx) * g;
+    }
+    dwdepth[i] = acc;
 }
 
 // ---- depth predictor tail ---------------------------------------------------------------------------------------------
@@ -165,13 +195,17 @@ depth_tail_fwd_kernel(const float* __restrict__ logits, const float* __restrict_
 }
 // backward: d_ip (npix, C), d_wd_ext (npix) = gradient reaching weighted_depth from elsewhere (the heads' depth-map lookup), or null.
 // demb (E, C) accumulated through a per-CTA shared-memory copy (the 61 rows are hit by every pixel), dlogits (npix, nb) written.
+// EMB = false: dlogits only (the embedding gradient comes from depth_tail_emb_grad_kernel).
+template <bool EMB = true>
 __global__ void __launch_bounds__(256)
 depth_tail_bwd_kernel(const float* __restrict__ logits, const float* __restrict__ bins, const float* __restrict__ emb,
                       const float* __restrict__ d_ip, const float* __restrict__ d_wd_ext, float* __restrict__ dlogits,
                       float* __restrict__ demb, long long npix, int nb, int E, int C, float dmax) {
     extern __shared__ float sacc[];                                // [E][C]
-    for (int i = threadIdx.x; i < E * C; i += blockDim.x) sacc[i] = 0.f;
-    __syncthreads();
+    if constexpr (EMB) {
+        for (int i = threadIdx.x; i < E * C; i += blockDim.x) sacc[i] = 0.f;
+        __syncthreads();
+    }
     const int lane = threadIdx.x & 31;
     const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
     // Embedding gradient: neighbouring pixels mostly fall into the same depth bin, so every warp walks a CONTIGUOUS pixel range and
@@ -224,7 +258,7 @@ depth_tail_bwd_kernel(const float* __restrict__ logits, const float* __restrict_
         const float f = floorf(x);
         const float delta = x - f;
         const int fi = (int)f, ci = min(fi + 1, E - 1);
-        if (fi != cur_f) {                                         // uniform across the warp
+        if (EMB && fi != cur_f) {                                  // uniform across the warp
             flush();
             cur_f = fi; cur_c = ci;
         }
@@ -239,9 +273,11 @@ depth_tail_bwd_kernel(const float* __restrict__ logits, const float* __restrict_
                 const float4 gg = *reinterpret_cast<const float4*>(g + ch);
                 const float4 a = *reinterpret_cast<const float4*>(e0 + ch), bb = *reinterpret_cast<const float4*>(e1 + ch);
                 dd += gg.x * (bb.x - a.x) + gg.y * (bb.y - a.y) + gg.z * (bb.z - a.z) + gg.w * (bb.w - a.w);
+                if constexpr (EMB) {
                 af[hh * 4 + 0] += gg.x * (1.f - delta); af[hh * 4 + 1] += gg.y * (1.f - delta);
                 af[hh * 4 + 2] += gg.z * (1.f - delta); af[hh * 4 + 3] += gg.w * (1.f - delta);
                 ac[hh * 4 + 0] += gg.x * delta; ac[hh * 4 + 1] += gg.y * delta; ac[hh * 4 + 2] += gg.z * delta; ac[hh * 4 + 3] += gg.w * delta;
+                }
             }
         }
 #pragma unroll
@@ -256,12 +292,82 @@ depth_tail_bwd_kernel(const float* __restrict__ logits, const float* __restrict_
             if (j < nb) dlogits[px * nb + j] = e[k] / se * (bins[j] - wd) * dwd;
         }
     }
-    flush();
-    __syncthreads();
-    for (int i = threadIdx.x; i < E * C; i += blockDim.x) {
-        const float a = sacc[i];
-        if (a != 0.f) atomicAdd(demb + i, a);
+    if constexpr (EMB) {
+        flush();
+        __syncthreads();
+        for (int i = threadIdx.x; i < E * C; i += blockDim.x) {
+            const float a = sacc[i];
+            if (a != 0.f) atomicAdd(demb + i, a);
+        }
     }
+}
+
+// Reproducible embedding gradient: CTA (row e, r) of a cluster of 8 sums, per channel, the pixels of its fixed range
+// [r*npix/8, (r+1)*npix/8) in pixel order, and cluster rank 0 adds the 8 partial rows in rank order through distributed shared
+// memory; demb is fully written.  The weighted depth of each pixel (floor index and fraction) is recomputed from the logits by a
+// warp, with the forward's lane mapping and reduction order, 256 pixels at a time.
+constexpr int DT_CLUSTER = 8;
+__global__ void __cluster_dims__(1, DT_CLUSTER, 1) __launch_bounds__(256)
+depth_tail_emb_grad_kernel(const float* __restrict__ logits, const float* __restrict__ bins, const float* __restrict__ d_ip,
+                           float* __restrict__ demb, long long npix, int nb, int E, int C, float dmax) {
+    __shared__ float part[256];
+    __shared__ float s_x[256];                                     // clamped weighted depth of the chunk's pixels
+    cg::cluster_group cluster = cg::this_cluster();
+    const int e = blockIdx.x, rank = (int)cluster.block_rank();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, ch = threadIdx.x;
+    const long long p0 = npix * rank / DT_CLUSTER, p1 = npix * (rank + 1) / DT_CLUSTER;
+    float acc = 0.f;
+    for (long long base = p0; base < p1; base += 256) {
+        const int n = (int)min(256LL, p1 - base);
+        __syncthreads();                                           // the previous chunk is consumed
+        for (int k = wid; k < n; k += 8) {
+            const float* lg = logits + (base + k) * nb;
+            float v[3], mx = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                const int b = lane + 32 * j;
+                v[j] = b < nb ? lg[b] : -INFINITY;
+                mx = fmaxf(mx, v[j]);
+            }
+#pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+            float se = 0.f, sw = 0.f;
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                const int b = lane + 32 * j;
+                const float ex = b < nb ? expf(v[j] - mx) : 0.f;
+                se += ex;
+                sw += b < nb ? ex * bins[b] : 0.f;
+            }
+#pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) {
+                se += __shfl_xor_sync(0xffffffffu, se, o);
+                sw += __shfl_xor_sync(0xffffffffu, sw, o);
+            }
+            if (lane == 0) s_x[k] = fminf(fmaxf(sw / se, 0.f), dmax);
+        }
+        __syncthreads();
+        if (ch < C) {
+            for (int k = 0; k < n; ++k) {
+                const float x = s_x[k];
+                const float f = floorf(x);
+                const float delta = x - f;
+                const int fi = (int)f, ci = min(fi + 1, E - 1);
+                if (fi != e && ci != e) continue;
+                const float gg = d_ip[(base + k) * C + ch];
+                if (fi == e) acc += gg * (1.f - delta);
+                if (ci == e) acc += gg * delta;
+            }
+        }
+    }
+    part[ch] = acc;
+    cluster.sync();
+    if (rank == 0 && ch < C) {
+        float a = 0.f;
+        for (int r = 0; r < DT_CLUSTER; ++r) a += cluster.map_shared_rank(part, r)[ch];
+        demb[(size_t)e * C + ch] = a;
+    }
+    cluster.sync();
 }
 
 // ---- mean of three maps, scale -------------------------------------------------------------------------------------------
@@ -303,6 +409,28 @@ __global__ void __launch_bounds__(256) sum_mean_sq_fwd_kernel(const __grid_const
         for (int w = 0; w < 8; ++w) s += part[w];
         atomicAdd(loss, s / (float)n);
     }
+}
+// Reproducible mode: ONE CTA adds the tensors in order, each as a fixed-stride per-thread sum, a fixed warp tree and the warps in order.
+__global__ void __launch_bounds__(1024) sum_mean_sq_fwd_ordered_kernel(const __grid_constant__ LossTable tb, float* __restrict__ loss) {
+    __shared__ float part[32];
+    float total = 0.f;
+    for (int k = 0; k < tb.count; ++k) {
+        const float* __restrict__ x = tb.x[k];
+        const long long n = tb.n[k];
+        float acc = 0.f;
+        for (long long i = threadIdx.x; i < n; i += blockDim.x) acc = fmaf(x[i], x[i], acc);
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            float s = 0.f;
+            for (int w = 0; w < 32; ++w) s += part[w];
+            total += s / (float)n;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *loss = total;
 }
 __global__ void __launch_bounds__(256) sum_mean_sq_bwd_kernel(const __grid_constant__ LossTable tb, const float* __restrict__ dloss) {
     const int k = blockIdx.y;
@@ -348,11 +476,20 @@ int mdb_head_depth_backward_f32(const float* dout, const float* coord, const flo
     if (B <= 0 || N < 0 || H <= 0 || W <= 0) return MDB_EINVAL;
     if (!dwdepth) return MDB_EINVAL;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (mdb_get_deterministic()) {                   // reproducible mode: per-query gradients, then the map gradient in gather form
+        if (N > 0) {
+            if (!dout || !coord || !size3d || !depth_reg || !calibs || !img_sizes || !dcoord || !dsize3d || !dreg) return MDB_EINVAL;
+            head_depth_bwd_kernel<false><<<(B * N + 127) / 128, 128, 0, stream>>>(dout, coord, size3d, depth_reg, calibs, img_sizes, dcoord,
+                                                                                dsize3d, dreg, dwdepth, B, N, H, W);
+        }
+        head_depth_bwd_gather_kernel<<<(B * H * W + 127) / 128, 128, 0, stream>>>(dout, coord, dwdepth, B, N, H, W);
+        return (int)cudaGetLastError();
+    }
     cudaError_t e = cudaMemsetAsync(dwdepth, 0, sizeof(float) * (size_t)B * H * W, stream);
     if (e != cudaSuccess) return (int)e;
     if (N == 0) return 0;
     if (!dout || !coord || !size3d || !depth_reg || !calibs || !img_sizes || !dcoord || !dsize3d || !dreg) return MDB_EINVAL;
-    head_depth_bwd_kernel<<<(B * N + 127) / 128, 128, 0, stream>>>(dout, coord, size3d, depth_reg, calibs, img_sizes, dcoord, dsize3d, dreg,
+    head_depth_bwd_kernel<true><<<(B * N + 127) / 128, 128, 0, stream>>>(dout, coord, size3d, depth_reg, calibs, img_sizes, dcoord, dsize3d, dreg,
                                                                    dwdepth, B, N, H, W);
     return (int)cudaGetLastError();
 }
@@ -371,19 +508,27 @@ int mdb_depth_tail_backward_f32(const float* logits, const float* bins, const fl
                                 float* dlogits, float* demb, long long npix, int nb, int E, int C, float dmax, void* stream_) {
     if (npix < 0 || nb <= 0 || nb > kMaxBins || E <= 0 || C <= 0 || C % 4 || C > 256 || (size_t)E * C * 4 > 96 * 1024) return MDB_EINVAL;
     if (!demb) return MDB_EINVAL;
+    if (mdb_get_deterministic()) {                   // reproducible mode: dlogits, then the embedding gradient in a fixed order
+        cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+        if (npix == 0) return (int)cudaMemsetAsync(demb, 0, sizeof(float) * (size_t)E * C, stream);
+        if (!logits || !bins || !emb || !d_ip || !dlogits) return MDB_EINVAL;
+        depth_tail_bwd_kernel<false><<<grid_cap(npix * 32, 256, num_sms()), 256, 0, stream>>>(logits, bins, emb, d_ip, d_wd_ext, dlogits,
+                                                                                               nullptr, npix, nb, E, C, dmax);
+        depth_tail_emb_grad_kernel<<<dim3(E, DT_CLUSTER), 256, 0, stream>>>(logits, bins, d_ip, demb, npix, nb, E, C, dmax);
+        return (int)cudaGetLastError();
+    }
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     cudaError_t e = cudaMemsetAsync(demb, 0, sizeof(float) * (size_t)E * C, stream);
     if (e != cudaSuccess) return (int)e;
     if (npix == 0) return 0;
     if (!logits || !bins || !emb || !d_ip || !dlogits) return MDB_EINVAL;
     const int smem = E * C * 4;
-    e = set_max_dynamic_smem(depth_tail_bwd_kernel, 96 * 1024);
+    e = set_max_dynamic_smem(depth_tail_bwd_kernel<true>, 96 * 1024);
     if (e != cudaSuccess) return (int)e;
-    depth_tail_bwd_kernel<<<grid_cap(npix * 32, 256, num_sms()), 256, smem, stream>>>(logits, bins, emb, d_ip, d_wd_ext, dlogits, demb, npix, nb, E, C,
+    depth_tail_bwd_kernel<true><<<grid_cap(npix * 32, 256, num_sms()), 256, smem, stream>>>(logits, bins, emb, d_ip, d_wd_ext, dlogits, demb, npix, nb, E, C,
                                                                                        dmax);
     return (int)cudaGetLastError();
 }
-
 int mdb_mean3_f32(const float* a, const float* b, const float* c, float* out, long long n, void* stream) {
     if (n < 0 || n % 4) return MDB_EINVAL;
     if (n == 0) return 0;
@@ -416,7 +561,10 @@ int mdb_sum_mean_squares_forward_f32(int count, const float* const* x, const lon
         tb.x[k] = x[k]; tb.g[k] = nullptr; tb.n[k] = n[k];
         if (n[k] > nmax) nmax = n[k];
     }
-    sum_mean_sq_fwd_kernel<<<dim3(grid_cap(nmax, 256 * 8, 64), count), 256, 0, stream>>>(tb, loss);
+    if (mdb_get_deterministic())                    // reproducible mode: one CTA, tensors and partial sums in a fixed order
+        sum_mean_sq_fwd_ordered_kernel<<<1, 1024, 0, stream>>>(tb, loss);
+    else
+        sum_mean_sq_fwd_kernel<<<dim3(grid_cap(nmax, 256 * 8, 64), count), 256, 0, stream>>>(tb, loss);
     return (int)cudaGetLastError();
 }
 int mdb_sum_mean_squares_backward_f32(int count, const float* const* x, float* const* g, const long long* n, const float* dloss,

@@ -3,6 +3,7 @@
 // depth_predictor/transformer.py:60-65) and GroupNorm(32, C) on NHWC activations (monodetr.py:83-91,
 // depth_predictor.py:29-45, optionally fused with ReLU), forward and backward, for sm_90a.
 // These are HBM-bound passes: one read of each input, one write of each output, fp32 statistics.
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -84,8 +85,9 @@ add_ln_fwd_kernel(const float* __restrict__ x, const float* __restrict__ res, co
     }
 }
 
-// dz = LN backward wrt z = x + drop(res); dres = dz * mask/(1-p) (written only when dres != dz semantics needed)
-template <int NV>
+// dz = LN backward wrt z = x + drop(res); dres = dz * mask/(1-p) (written only when dres != dz semantics needed).
+// PGRAD = false (reproducible mode): dgamma / dbeta are left to ln_param_grad_kernel.
+template <int NV, bool PGRAD = true>
 __global__ void __launch_bounds__(LN_THREADS)
 add_ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ res,
                   const float* __restrict__ gamma, const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
@@ -132,8 +134,10 @@ add_ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, con
             gy[i] = make_float4(d.x * g[i].x, d.y * g[i].y, d.z * g[i].z, d.w * g[i].w);
             s1 += gy[i].x + gy[i].y + gy[i].z + gy[i].w;
             s2 += gy[i].x * xh[i].x + gy[i].y * xh[i].y + gy[i].z * xh[i].z + gy[i].w * xh[i].w;
-            adg[i].x += d.x * xh[i].x; adg[i].y += d.y * xh[i].y; adg[i].z += d.z * xh[i].z; adg[i].w += d.w * xh[i].w;
-            adb[i].x += d.x; adb[i].y += d.y; adb[i].z += d.z; adb[i].w += d.w;
+            if constexpr (PGRAD) {
+                adg[i].x += d.x * xh[i].x; adg[i].y += d.y * xh[i].y; adg[i].z += d.z * xh[i].z; adg[i].w += d.w * xh[i].w;
+                adb[i].x += d.x; adb[i].y += d.y; adb[i].z += d.z; adb[i].w += d.w;
+            }
         }
         s1 = warp_sum(s1) * (1.f / C);
         s2 = warp_sum(s2) * (1.f / C);
@@ -152,20 +156,22 @@ add_ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, con
             }
         }
     }
-    // reduce dgamma / dbeta over the 8 warps of the CTA, then one atomic per channel per CTA
+    if constexpr (PGRAD) {
+        // reduce dgamma / dbeta over the 8 warps of the CTA, then one atomic per channel per CTA
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const int c = (i * 32 + lane) * 4;
-        s_dg[wid][c] = adg[i].x; s_dg[wid][c + 1] = adg[i].y; s_dg[wid][c + 2] = adg[i].z; s_dg[wid][c + 3] = adg[i].w;
-        s_db[wid][c] = adb[i].x; s_db[wid][c + 1] = adb[i].y; s_db[wid][c + 2] = adb[i].z; s_db[wid][c + 3] = adb[i].w;
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < C; c += LN_THREADS) {
-        float a = 0.f, b = 0.f;
+        for (int i = 0; i < NV; ++i) {
+            const int c = (i * 32 + lane) * 4;
+            s_dg[wid][c] = adg[i].x; s_dg[wid][c + 1] = adg[i].y; s_dg[wid][c + 2] = adg[i].z; s_dg[wid][c + 3] = adg[i].w;
+            s_db[wid][c] = adb[i].x; s_db[wid][c + 1] = adb[i].y; s_db[wid][c + 2] = adb[i].z; s_db[wid][c + 3] = adb[i].w;
+        }
+        __syncthreads();
+        for (int c = threadIdx.x; c < C; c += LN_THREADS) {
+            float a = 0.f, b = 0.f;
 #pragma unroll
-        for (int w = 0; w < LN_THREADS / 32; ++w) { a += s_dg[w][c]; b += s_db[w][c]; }
-        atomicAdd(dgamma + c, a);
-        atomicAdd(dbeta + c, b);
+            for (int w = 0; w < LN_THREADS / 32; ++w) { a += s_dg[w][c]; b += s_db[w][c]; }
+            atomicAdd(dgamma + c, a);
+            atomicAdd(dbeta + c, b);
+        }
     }
 }
 
@@ -333,6 +339,175 @@ gn_bwd_apply_kernel(const float* __restrict__ dy, const float* __restrict__ x, c
     }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Reproducible mode (mdb_set_deterministic(1)): every output element has exactly one writer that adds its terms in an order
+// fixed by the problem shape alone (never by the SM count or the scheduling).
+// ---------------------------------------------------------------------------------------------------
+namespace cg = cooperative_groups;
+constexpr int LNP_CLUSTER = 8;   // CTAs per 32-column slab; cluster rank r owns rows [r*M/8, (r+1)*M/8)
+
+// LayerNorm dgamma / dbeta: CTA (slab, r) sums d * xhat and d over its rows (warp w, row group sub = lane/8: rows
+// r0 + 4w + sub, step 32; lane & 7 = float4 column quad), reduces its 8 warps in order in shared memory, and cluster rank 0
+// adds the 8 CTA totals in rank order through distributed shared memory.  C = 256: 64 CTAs, no global scratch.
+__global__ void __cluster_dims__(1, LNP_CLUSTER, 1) __launch_bounds__(256)
+ln_param_grad_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ res,
+                     const float* __restrict__ mean_in, const float* __restrict__ rstd_in, float* __restrict__ dgamma,
+                     float* __restrict__ dbeta, long long M, int C, float drop_p, const unsigned long long* __restrict__ seed_ptr,
+                     unsigned long long site, int accumulate) {
+    __shared__ float4 s_g[8][8], s_b[8][8];
+    __shared__ float s_tg[32], s_tb[32];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, sub = lane >> 3, q = lane & 7;
+    const int c0 = blockIdx.x * 32 + q * 4;
+    const int rank = (int)cluster.block_rank();
+    const long long r0 = M * rank / LNP_CLUSTER, r1 = M * (rank + 1) / LNP_CLUSTER;
+    const unsigned long long seed = (drop_p > 0.f) ? (*seed_ptr + site * 0x9E3779B97F4A7C15ull) : 0ull;
+    const float inv_keep = 1.f / (1.f - drop_p);
+    float4 dg = make_float4(0.f, 0.f, 0.f, 0.f), db = dg;
+    for (long long row = r0 + wid * 4 + sub; row < r1; row += 32) {
+        const size_t off = (size_t)row * C + c0;
+        float4 z = *reinterpret_cast<const float4*>(x + off);
+        if (res) {
+            float4 r = *reinterpret_cast<const float4*>(res + off);
+            if (drop_p > 0.f) {
+                float u[4];
+                mdb::rng_uniform4(seed, off >> 2, u);
+                r.x = u[0] >= drop_p ? r.x * inv_keep : 0.f;
+                r.y = u[1] >= drop_p ? r.y * inv_keep : 0.f;
+                r.z = u[2] >= drop_p ? r.z * inv_keep : 0.f;
+                r.w = u[3] >= drop_p ? r.w * inv_keep : 0.f;
+            }
+            z.x += r.x; z.y += r.y; z.z += r.z; z.w += r.w;
+        }
+        const float mean = mean_in[row], rstd = rstd_in[row];
+        const float4 d = *reinterpret_cast<const float4*>(dy + off);
+        dg.x += d.x * ((z.x - mean) * rstd); dg.y += d.y * ((z.y - mean) * rstd);
+        dg.z += d.z * ((z.z - mean) * rstd); dg.w += d.w * ((z.w - mean) * rstd);
+        db.x += d.x; db.y += d.y; db.z += d.z; db.w += d.w;
+    }
+#pragma unroll
+    for (int o = 8; o <= 16; o <<= 1) {                              // the 4 row groups of the warp
+        dg.x += __shfl_xor_sync(0xffffffffu, dg.x, o); dg.y += __shfl_xor_sync(0xffffffffu, dg.y, o);
+        dg.z += __shfl_xor_sync(0xffffffffu, dg.z, o); dg.w += __shfl_xor_sync(0xffffffffu, dg.w, o);
+        db.x += __shfl_xor_sync(0xffffffffu, db.x, o); db.y += __shfl_xor_sync(0xffffffffu, db.y, o);
+        db.z += __shfl_xor_sync(0xffffffffu, db.z, o); db.w += __shfl_xor_sync(0xffffffffu, db.w, o);
+    }
+    if (sub == 0) { s_g[wid][q] = dg; s_b[wid][q] = db; }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        float a = 0.f, b = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+            a += reinterpret_cast<const float*>(s_g[w])[threadIdx.x];
+            b += reinterpret_cast<const float*>(s_b[w])[threadIdx.x];
+        }
+        s_tg[threadIdx.x] = a;
+        s_tb[threadIdx.x] = b;
+    }
+    cluster.sync();
+    if (rank == 0 && threadIdx.x < 32) {
+        float a = 0.f, b = 0.f;
+        for (int r = 0; r < LNP_CLUSTER; ++r) {
+            a += cluster.map_shared_rank(s_tg, r)[threadIdx.x];
+            b += cluster.map_shared_rank(s_tb, r)[threadIdx.x];
+        }
+        const int c = blockIdx.x * 32 + threadIdx.x;
+        dgamma[c] = accumulate ? dgamma[c] + a : a;
+        dbeta[c] = accumulate ? dbeta[c] + b : b;
+    }
+    cluster.sync();                                                  // keep every CTA's shared memory alive until rank 0 has read it
+}
+
+// GroupNorm statistics: one CTA per (group, image) sums all HW pixels of its C/G channels (thread t: channel quad t % qpg,
+// pixels t / qpg + k * (256 / qpg)), then a fixed tree over the 256 partials in double; stats written directly.
+__device__ __forceinline__ void tree_sum2(double (*sh)[GN_THREADS]) {
+#pragma unroll
+    for (int o = GN_THREADS / 2; o > 0; o >>= 1) {
+        if (threadIdx.x < o) { sh[0][threadIdx.x] += sh[0][threadIdx.x + o]; sh[1][threadIdx.x] += sh[1][threadIdx.x + o]; }
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(GN_THREADS)
+gn_stats_group_kernel(const float* __restrict__ x, double* __restrict__ stats, int HW, int C, int G) {
+    const int g = blockIdx.x, b = blockIdx.y;
+    const int qpg = C / G / 4, q = threadIdx.x % qpg, pl = threadIdx.x / qpg, pls = GN_THREADS / qpg;
+    const float* xp = x + (size_t)b * HW * C + g * (C / G) + q * 4;
+    float s = 0.f, ss = 0.f;
+    for (int p = pl; p < HW; p += pls) {
+        const float4 v = *reinterpret_cast<const float4*>(xp + (size_t)p * C);
+        s += v.x + v.y + v.z + v.w;
+        ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+    }
+    __shared__ double sh[2][GN_THREADS];
+    sh[0][threadIdx.x] = s;
+    sh[1][threadIdx.x] = ss;
+    __syncthreads();
+    tree_sum2(sh);
+    if (threadIdx.x == 0) {
+        stats[((size_t)b * G + g) * 2] = sh[0][0];
+        stats[((size_t)b * G + g) * 2 + 1] = sh[1][0];
+    }
+}
+
+// GroupNorm backward statistics and dgamma / dbeta: one CTA per group walks the images in order (stats of (b, g) written
+// directly after each image); each thread keeps its quad's dgamma / dbeta over all images and the CTA adds the 256 / qpg pixel
+// lanes in lane order.  B * HW * C / G elements per CTA.
+__global__ void __launch_bounds__(GN_THREADS)
+gn_bwd_group_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ y,
+                    const float* __restrict__ gamma, const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
+                    double* __restrict__ stats, float* __restrict__ dgamma, float* __restrict__ dbeta, int B, int HW, int C, int G,
+                    int relu) {
+    const int g = blockIdx.x;
+    const int qpg = C / G / 4, q = threadIdx.x % qpg, pl = threadIdx.x / qpg, pls = GN_THREADS / qpg;
+    const int c0 = g * (C / G) + q * 4;
+    const float4 ga = *reinterpret_cast<const float4*>(gamma + c0);
+    __shared__ double sh[2][GN_THREADS];
+    __shared__ float4 shg[GN_THREADS], shb[GN_THREADS];
+    float4 dg = make_float4(0.f, 0.f, 0.f, 0.f), db = dg;
+    for (int b = 0; b < B; ++b) {
+        const float mean = mean_in[(size_t)b * G + g], rstd = rstd_in[(size_t)b * G + g];
+        float s1 = 0.f, s2 = 0.f;
+        for (int p = pl; p < HW; p += pls) {
+            const size_t off = ((size_t)b * HW + p) * C + c0;
+            float4 d = *reinterpret_cast<const float4*>(dy + off);
+            if (relu) {
+                const float4 o = *reinterpret_cast<const float4*>(y + off);
+                d.x = o.x > 0.f ? d.x : 0.f; d.y = o.y > 0.f ? d.y : 0.f; d.z = o.z > 0.f ? d.z : 0.f; d.w = o.w > 0.f ? d.w : 0.f;
+            }
+            const float4 v = *reinterpret_cast<const float4*>(x + off);
+            const float4 xh = make_float4((v.x - mean) * rstd, (v.y - mean) * rstd, (v.z - mean) * rstd, (v.w - mean) * rstd);
+            s1 += d.x * ga.x + d.y * ga.y + d.z * ga.z + d.w * ga.w;
+            s2 += d.x * ga.x * xh.x + d.y * ga.y * xh.y + d.z * ga.z * xh.z + d.w * ga.w * xh.w;
+            dg.x += d.x * xh.x; dg.y += d.y * xh.y; dg.z += d.z * xh.z; dg.w += d.w * xh.w;
+            db.x += d.x; db.y += d.y; db.z += d.z; db.w += d.w;
+        }
+        sh[0][threadIdx.x] = s1;
+        sh[1][threadIdx.x] = s2;
+        __syncthreads();
+        tree_sum2(sh);
+        if (threadIdx.x == 0) {
+            stats[((size_t)b * G + g) * 2] = sh[0][0];
+            stats[((size_t)b * G + g) * 2 + 1] = sh[1][0];
+        }
+        __syncthreads();
+    }
+    shg[threadIdx.x] = dg;
+    shb[threadIdx.x] = db;
+    __syncthreads();
+    if (threadIdx.x < qpg) {
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f), c = a;
+        for (int l = 0; l < pls; ++l) {
+            const float4 t = shg[l * qpg + threadIdx.x], u = shb[l * qpg + threadIdx.x];
+            a.x += t.x; a.y += t.y; a.z += t.z; a.w += t.w;
+            c.x += u.x; c.y += u.y; c.z += u.z; c.w += u.w;
+        }
+        const int cc = g * (C / G) + threadIdx.x * 4;
+        *reinterpret_cast<float4*>(dgamma + cc) = a;
+        *reinterpret_cast<float4*>(dbeta + cc) = c;
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -368,6 +543,28 @@ int mdb_add_layernorm_backward_f32(const float* dy, const float* x, const float*
     if (C % 128 || C > 512) return MDB_EUNSUPPORTED;   // smem staging of dgamma/dbeta: 8 warps x C x 2 floats
     if (drop_p > 0.f && (!seed || !dres)) return MDB_EINVAL;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (mdb_get_deterministic()) {
+        // reproducible mode: dx / dres as below without the parameter gradients, then one fixed-order pass for dgamma / dbeta
+        if (M == 0) {
+            if (!accumulate) {
+                cudaMemsetAsync(dgamma, 0, sizeof(float) * C, stream);
+                cudaMemsetAsync(dbeta, 0, sizeof(float) * C, stream);
+            }
+            return 0;
+        }
+        const int grid = grid_cap(M, LN_THREADS / 32, num_sms() * 4);
+#define MDB_LN_BWD_NP(NV) add_ln_bwd_kernel<NV, false><<<grid, LN_THREADS, 0, stream>>>(dy, x, res, gamma, mean, rstd, dx, dres, dgamma, dbeta, M, drop_p, seed, site)
+        switch (C / 128) {
+            case 1: MDB_LN_BWD_NP(1); break;
+            case 2: MDB_LN_BWD_NP(2); break;
+            case 4: MDB_LN_BWD_NP(4); break;
+            default: return MDB_EUNSUPPORTED;
+        }
+#undef MDB_LN_BWD_NP
+        ln_param_grad_kernel<<<dim3(C / 32, LNP_CLUSTER), 256, 0, stream>>>(dy, x, res, mean, rstd, dgamma, dbeta, M, C, drop_p, seed,
+                                                                            site, accumulate);
+        return (int)cudaGetLastError();
+    }
     if (!accumulate) {
         cudaMemsetAsync(dgamma, 0, sizeof(float) * C, stream);
         cudaMemsetAsync(dbeta, 0, sizeof(float) * C, stream);
@@ -391,6 +588,13 @@ int mdb_groupnorm_forward_f32(const float* x, const float* gamma, const float* b
     if (!x || !gamma || !beta || !y || !mean || !rstd || !stats_ws || B <= 0 || HW <= 0) return MDB_EINVAL;
     if (C % 4 || (GN_THREADS % (C / 4)) || C % G || (C / G) % 4 || G > GN_THREADS) return MDB_EUNSUPPORTED;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (mdb_get_deterministic()) {                   // reproducible mode: one CTA per (group, image) writes its sums
+        if (GN_THREADS % (C / G / 4)) return MDB_EUNSUPPORTED;
+        gn_stats_group_kernel<<<dim3(G, B), GN_THREADS, 0, stream>>>(x, stats_ws, HW, C, G);
+        gn_apply_kernel<<<grid_cap((long long)B * HW * C / 4, GN_THREADS, num_sms() * 16), GN_THREADS, 0, stream>>>(x, stats_ws, gamma, beta, y,
+                                                                                                     mean, rstd, B, HW, C, G, eps, relu);
+        return (int)cudaGetLastError();
+    }
     cudaMemsetAsync(stats_ws, 0, sizeof(double) * B * G * 2, stream);
     int blocks = (HW + 255) / 256;
     if (blocks > 64) blocks = 64;
@@ -409,6 +613,13 @@ int mdb_groupnorm_backward_f32(const float* dy, const float* x, const float* y, 
     if (relu && !y) return MDB_EINVAL;
     if (C % 4 || (GN_THREADS % (C / 4)) || C % G || (C / G) % 4 || G > GN_THREADS) return MDB_EUNSUPPORTED;
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (mdb_get_deterministic()) {                   // reproducible mode: one CTA per group, images and pixels in a fixed order
+        if (GN_THREADS % (C / G / 4)) return MDB_EUNSUPPORTED;
+        gn_bwd_group_kernel<<<G, GN_THREADS, 0, stream>>>(dy, x, y, gamma, mean, rstd, stats_ws, dgamma, dbeta, B, HW, C, G, relu);
+        gn_bwd_apply_kernel<<<grid_cap((long long)B * HW * C / 4, GN_THREADS, num_sms() * 16), GN_THREADS, 0, stream>>>(dy, x, y, gamma, mean, rstd,
+                                                                                                        stats_ws, dx, B, HW, C, G, relu);
+        return (int)cudaGetLastError();
+    }
     cudaMemsetAsync(stats_ws, 0, sizeof(double) * B * G * 2, stream);
     cudaMemsetAsync(dgamma, 0, sizeof(float) * C, stream);
     cudaMemsetAsync(dbeta, 0, sizeof(float) * C, stream);

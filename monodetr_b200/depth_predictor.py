@@ -8,7 +8,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from . import functional as Fn
+from . import _lib, functional as Fn
 
 
 class TransformerEncoderLayer(nn.Module):
@@ -67,6 +67,14 @@ class _ConvGN(nn.Sequential):
         return Fn.groupnorm_nhwc(y, gn.weight, gn.bias, gn.num_groups, gn.eps, relu)
 
 
+def library_resize(x):
+    """Whether the 1/32 map is resized with the library's kernel (mdb_upsample_bilinear_nhwc_*) instead of F.interpolate: in
+    reproducible mode, for a map on a CUDA device, because torch's CUDA backward of the bilinear resize scatters with atomics
+    (and raises under torch.use_deterministic_algorithms(True)).  Its CPU backward -- reached only by the host-logic tests,
+    which drive the model with CPU tensors -- is deterministic, and the default mode keeps F.interpolate everywhere."""
+    return _lib.deterministic() and x.device.type == "cuda"
+
+
 class DepthPredictor(nn.Module):
     def __init__(self, model_cfg):
         super().__init__()
@@ -96,7 +104,10 @@ class DepthPredictor(nn.Module):
         depth_pos_embed_ip (B, HW, C)  -- the reference's (:91) tensors in channels-last layout."""
         assert len(feature) == 4
         src_16 = self.proj(feature[1])
-        up = F.interpolate(feature[2].permute(0, 3, 1, 2), size=src_16.shape[1:3], mode="bilinear").permute(0, 2, 3, 1)
+        if library_resize(feature[2]):
+            up = Fn.upsample_bilinear_nhwc(feature[2], src_16.shape[1:3])
+        else:
+            up = F.interpolate(feature[2].permute(0, 3, 1, 2), size=src_16.shape[1:3], mode="bilinear").permute(0, 2, 3, 1)
         src_32 = self.upsample(up.contiguous())
         src_8 = self.downsample(feature[0])
         src = Fn.mean3(src_8, src_16, src_32)

@@ -642,7 +642,9 @@ class _HeadDepth(Function):
         dout = dout.contiguous()
         dcoord, dsize, dreg = torch.empty_like(coord), torch.empty_like(size3d), torch.empty_like(depth_reg)
         dwd = torch.empty((B, H, W), dtype=torch.float32, device=dout.device)
-        _lib.call("mdb_head_depth_backward_f32", dout, coord, size3d, depth_reg, calibs, img_sizes, dcoord, dsize, dreg, dwd, B, N, H, W)
+        # reproducible mode: the map gradient is a second (gather) launch
+        _lib.call("mdb_head_depth_backward_f32", dout, coord, size3d, depth_reg, calibs, img_sizes, dcoord, dsize, dreg, dwd, B, N, H, W,
+                  launches=2 if _lib.deterministic() else 1)
         return dcoord, dsize, dreg, dwd, None, None
 
 
@@ -676,12 +678,41 @@ class _DepthTail(Function):
         dwd = None if dwd is None else dwd.contiguous()
         dlogits = torch.empty_like(logits)
         demb = torch.empty_like(embc)
-        _lib.call("mdb_depth_tail_backward_f32", logits, bins, embc, dip, dwd, dlogits, demb, npix, nb, E, C, dmax)
+        # reproducible mode: the embedding gradient is a second, fixed-order launch
+        _lib.call("mdb_depth_tail_backward_f32", logits, bins, embc, dip, dwd, dlogits, demb, npix, nb, E, C, dmax,
+                  launches=2 if _lib.deterministic() else 1)
         return dlogits, None, demb, None
 
 
 def depth_tail(logits, bins, emb, dmax):
     return _DepthTail.apply(logits, bins, emb, dmax)
+
+
+class _UpsampleBilinear(Function):
+    """F.interpolate(x, size, mode="bilinear", align_corners=False) on an NHWC map (B, H, W, C) -> (B, Ho, Wo, C); the backward is a
+    gather (no atomics), so it is bit-reproducible."""
+
+    @staticmethod
+    def forward(ctx, x, Ho, Wo):
+        x = x.contiguous()
+        B, H, W, C = x.shape
+        y = torch.empty((B, Ho, Wo, C), dtype=torch.float32, device=x.device)
+        _lib.call("mdb_upsample_bilinear_nhwc_forward_f32", x, y, B, H, W, Ho, Wo, C)
+        ctx.meta = (B, H, W, Ho, Wo, C)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        B, H, W, Ho, Wo, C = ctx.meta
+        dx = torch.empty((B, H, W, C), dtype=torch.float32, device=dy.device)
+        _lib.call("mdb_upsample_bilinear_nhwc_backward_f32", dy.contiguous(), dx, B, H, W, Ho, Wo, C)
+        return dx, None, None
+
+
+def upsample_bilinear_nhwc(x, size):
+    """Bilinear resize of an NHWC map to size = (Ho, Wo), torch's align_corners=False rule."""
+    return _UpsampleBilinear.apply(x, int(size[0]), int(size[1]))
 
 
 class _Mean3(Function):

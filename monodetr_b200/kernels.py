@@ -106,8 +106,9 @@ def add_layernorm_backward(dy, x, res, gamma, mean, rstd, drop_p=0.0, site=0, se
     dgamma = torch.empty((C,), dtype=torch.float32, device=x.device)
     dbeta = torch.empty((C,), dtype=torch.float32, device=x.device)
     seed = (seed if seed is not None else seed_tensor(x.device)) if drop_p > 0 else None
+    # reproducible mode: a second, fixed-order launch computes dgamma / dbeta
     _lib.call("mdb_add_layernorm_backward_f32", dy, x, res, gamma, mean, rstd, dx, dres, dgamma, dbeta, M, C, float(drop_p), seed,
-              site, 0)
+              site, 0, launches=2 if _lib.deterministic() else 1)
     return dx, (dres if dres is not None else dx), dgamma, dbeta
 
 
