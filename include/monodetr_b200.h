@@ -353,6 +353,43 @@ int mdb_warp_affine_normalize_u8(const unsigned char* const* src, const int* src
                                  const unsigned char* flip, int B, int out_w, int out_h, const float* mean3, const float* std3, float* out,
                                  void* stream);
 
+/* ---- KITTI evaluation on the device (kitti_eval.cu) ----
+ * lib/datasets/kitti/kitti_eval_python/eval.py:9-412,614-644 (get_thresholds, clean_data, image_box_overlap, d3_box_overlap,
+ * compute_statistics_jit, fused_compute_statistics) and rotate_iou.py:17-330 (the rotated-box IoU).  The annotations of n_img images
+ * are packed in CSR form: gt_off / dt_off (n_img+1) int32 prefix sums of the per-image box counts, ov_off (n_img+1) int64 prefix
+ * sums of n_dt_b * n_gt_b (the per-image overlap blocks; n_ov = ov_off[n_img]).  max_gt / max_dt are the largest per-image counts
+ * (HOST values; above MDB_KITTI_MAX_BOXES -> MDB_EUNSUPPORTED).
+ *   gt_f (n_gt, MDB_KITTI_GT_COLS) fp64: bbox x0 y0 x1 y1, alpha, truncated, location x y z, dimensions l h w, rotation_y
+ *   gt_i (n_gt, 3) int32: occluded, class code, DontCare flag (name == "DontCare", case-sensitive)
+ *   dt_f (n_dt, MDB_KITTI_DT_COLS) fp64: bbox x0 y0 x1 y1, alpha, score, location x y z, dimensions l h w, rotation_y
+ *   dt_cls (n_dt) int32: class code
+ * A class code is the index of the lower-cased name in {car, pedestrian, cyclist, van, person_sitting, truck}, -1 for any other.
+ * overlaps (3, n_ov) fp64: metric 0 = 2-d IoU (fp64), 1 = bird's-eye-view IoU of [x, z, l, w, ry] (fp32 polygon clipping,
+ * widened), 2 = 3-d IoU (the fp32 BEV intersection times the fp64 height overlap, rounded to fp32); the block of image b starts at
+ * ov_off[b], detection-major (n_dt_b, n_gt_b).  No FMA contraction anywhere: 2-d overlaps are bit-identical to the reference. */
+#define MDB_KITTI_MAX_BOXES 1024       /* gt boxes, and detections, per image */
+#define MDB_KITTI_MAX_CLASSES 6
+#define MDB_KITTI_MAX_TOTAL_GT (1 << 22)
+#define MDB_KITTI_NUM_THRESH 41        /* score thresholds (sample points) per configuration */
+#define MDB_KITTI_GT_COLS 13
+#define MDB_KITTI_DT_COLS 13
+int mdb_kitti_overlaps(const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int max_gt, int max_dt,
+                       long long n_ov, const double* gt_f, const double* dt_f, double* overlaps, void* stream);
+/* Bytes of scratch mdb_kitti_eval needs (negative = MDB_E*): about n_cfg * 8 * next_pow2(n_gt) for the score sort, plus
+ * n_cfg * 41 * n_img * 8 when compute_aos, plus per-box flags; n_cfg = 18 * n_cls. */
+long long mdb_kitti_eval_workspace_bytes(int n_img, int n_gt, int n_dt, int n_cls, int compute_aos);
+/* Every configuration cfg = ((metric * n_cls + m) * 3 + difficulty) * 2 + k of the classes `classes` (n_cls int32, codes as above)
+ * in one call: clean_data, the TP scores (compute_fp=False), the score thresholds, then tp / fp / fn / AOS similarity at each
+ * threshold (compute_fp=True).  min_overlaps (2, 3, n_cls) fp64 = the reference's min_overlaps[:, :, current_classes].
+ * result (n_cfg, 1 + 4 * MDB_KITTI_NUM_THRESH) fp64: [number of thresholds T, then (tp, fp, fn, similarity) per threshold]; rows
+ * t >= T are zero.  T > MDB_KITTI_NUM_THRESH is reported as is (the reference fails on such input).  similarity is summed per
+ * image in gt order and over images in image order, only for metric 0 with compute_aos.  n_img >= 1.  Five kernel launches, no float atomics:
+ * the result is the same in both reproducible modes.  workspace: at least mdb_kitti_eval_workspace_bytes (else MDB_EWORKSPACE). */
+int mdb_kitti_eval(const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int n_gt, int n_dt, int max_gt,
+                   int max_dt, long long n_ov, const double* gt_f, const int* gt_i, const double* dt_f, const int* dt_cls,
+                   const double* overlaps, const int* classes, const double* min_overlaps, int n_cls, int compute_aos,
+                   void* workspace, long long workspace_bytes, double* result, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

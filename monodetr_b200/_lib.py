@@ -78,8 +78,13 @@ SIGNATURES = {
     "mdb_warp_affine_normalize_u8": [_PTR] * 5 + [c_int] * 3 + [_PTR] * 4,
     "mdb_extract_dets_f32": [_PTR] * 5 + [c_int] * 4 + [_PTR, _PTR],
     "mdb_decode_dets_f32": [_PTR] * 4 + [c_int] * 3 + [c_float, _PTR, _PTR, _PTR],
+    "mdb_kitti_overlaps": [_PTR] * 3 + [c_int] * 3 + [ctypes.c_longlong] + [_PTR] * 4,
+    "mdb_kitti_eval_workspace_bytes": [c_int] * 5,
+    "mdb_kitti_eval": [_PTR] * 3 + [c_int] * 5 + [ctypes.c_longlong] + [_PTR] * 7 + [c_int] * 2 + [_PTR, ctypes.c_longlong]
+                      + [_PTR, _PTR],
 }
-_RESTYPES = {"mdb_error_string": ctypes.c_char_p, "mdb_conv2d_forward_workspace_bytes": ctypes.c_longlong}
+_RESTYPES = {"mdb_error_string": ctypes.c_char_p, "mdb_conv2d_forward_workspace_bytes": ctypes.c_longlong,
+             "mdb_kitti_eval_workspace_bytes": ctypes.c_longlong}
 
 
 def lib():
