@@ -353,6 +353,34 @@ int mdb_warp_affine_normalize_u8(const unsigned char* const* src, const int* src
                                  const unsigned char* flip, int B, int out_w, int out_h, const float* mean3, const float* std3, float* out,
                                  void* stream);
 
+/* Photometric distortion, the dataset's `aug_pd` step before the warp: kitti_dataset.py:136-138
+ * `pd(np.array(img).astype(np.float32)).astype(np.uint8)` with lib/datasets/kitti/pd.py:376-397.  One record per image holds the
+ * reference's random draws (drawn on the host; a step whose coin said no carries its neutral value, which gives the same bits as
+ * skipping it).  Record layout, 24 bytes, 4-byte aligned: */
+typedef struct mdb_photometric_params {
+    float brightness;   /* RandomBrightness delta, added to every channel first (0 = off) */
+    float contrast;     /* RandomContrast alpha, multiplies every channel (1 = off) */
+    float saturation;   /* RandomSaturation factor on S (1 = off) */
+    float hue;          /* RandomHue delta in degrees added to H, then > 360 -> -360, < 0 -> +360 (0 = off) */
+    int contrast_last;  /* 0: contrast, HSV, saturation, hue, BGR (pd[:-1]); 1: HSV, saturation, hue, BGR, contrast (pd[1:]) */
+    int perm;           /* RandomLightingNoise: out channel k = channel perms[perm][k] of pd.py:143-145, 0..5 (0 = identity = off) */
+} mdb_photometric_params;
+/* Per pixel in fp32, every scalar rounded to fp32 first: + brightness, then the colour steps in the record's order, then the
+ * channel permutation.  The RGB image is read as BGR (channel 0 is "B"), as the reference does.  The two cv2.cvtColor conversions
+ * are restated as cv2 4.13 computes them on float32 with AVX2 + FMA3: the hue of the last W % 8 pixels of each row comes from
+ * cv2's scalar loop, the others from its 8-wide vector loop, and the two round differently.  Those bits follow the reference's CPU
+ * dispatch; other cv2 builds or dispatch levels are not verified.  The final cast copies the REFERENCE'S QUIRK: numpy's float32 ->
+ * uint8 cast on x86 truncates toward zero and keeps the low 8 bits (290.3 -> 34, -5.7 -> 251), and values outside [0, 256) are
+ * common after a saturation or contrast factor above 1.
+ * src / src_wh / src_pitch: as mdb_warp_affine_normalize_u8 (all DEVICE arrays); params (B) DEVICE records; dst: DEVICE array of B
+ * device pointers to the 8-bit RGB outputs (W_b x H_b x 3, may not overlap the sources), dst_pitch (B) bytes per row (device).
+ * One launch; the library allocates nothing.  MDB_EINVAL for a null array or B outside 1..65535.  The records and sizes are read
+ * on the device, so the caller checks them: an image whose record has perm outside 0..5 or contrast_last outside 0..1, or whose
+ * size is not positive, is left unwritten (monodetr_b200.preprocess raises ValueError before launching). */
+int mdb_photometric_distort_u8(const unsigned char* const* src, const int* src_wh, const long long* src_pitch,
+                               const mdb_photometric_params* params, unsigned char* const* dst, const long long* dst_pitch, int B,
+                               void* stream);
+
 /* ---- KITTI evaluation on the device (kitti_eval.cu) ----
  * lib/datasets/kitti/kitti_eval_python/eval.py:9-412,614-644 (get_thresholds, clean_data, image_box_overlap, d3_box_overlap,
  * compute_statistics_jit, fused_compute_statistics) and rotate_iou.py:17-330 (the rotated-box IoU).  The annotations of n_img images

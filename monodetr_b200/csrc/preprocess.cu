@@ -7,11 +7,16 @@
 // (x - mean) / std (:159-161).
 // Arithmetic: coordinates and interpolation in fp64 exactly as PIL's C code (Geometry.c) so that the 8-bit value is
 // bit-identical; the float conversion in fp32 exactly as numpy's.  HBM-bound: 12 bytes written per output pixel.
+// Before it, when the dataset's `aug_pd` is on, a second kernel applies the reference's photometric distortion (:136-138,
+// pd.py:376-397) to every source image with its own host-drawn parameters and writes the 8-bit result to a caller buffer that the
+// warp then reads: pointwise, 3 bytes read and 3 written per source pixel.
 #include <cuda_runtime.h>
+#include <float.h>
 #include <math.h>
 #include <stdint.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 
 namespace {
 
@@ -57,7 +62,115 @@ __global__ void __launch_bounds__(256) warp_affine_normalize_kernel(const unsign
     o[2 * plane] = __fdiv_rn(__fsub_rn(__fdiv_rn(v[2], 255.f), mean.z), stdv.z);
 }
 
+// ---- photometric distortion (lib/datasets/kitti/pd.py:376-397 as called at kitti_dataset.py:136-138) ----------------------------
+// cv2.cvtColor BGR<->HSV on float32 as the reference's cv2 runs it (AVX2 + FMA3): a vector loop over 8 pixels and a scalar loop
+// over the last W % 8 pixels of each row, which round the hue differently.  Every operation is an explicit _rn intrinsic so that
+// nvcc contracts nothing the reference does not.
+constexpr int kHsvSimdWidth = 8;
+
+__device__ __forceinline__ void bgr_to_hsv(float b, float g, float r, bool scalar_tail, float& h, float& s, float& v) {
+    v = fmaxf(fmaxf(r, g), b);
+    const float vmin = fminf(fminf(r, g), b);
+    const float diff = __fsub_rn(v, vmin);
+    s = __fdiv_rn(diff, __fadd_rn(fabsf(v), FLT_EPSILON));
+    const float dd = __fadd_rn(diff, FLT_EPSILON);
+    float num, off;
+    if (r == v) { num = __fsub_rn(g, b); off = 0.f; }
+    else if (g == v) { num = __fsub_rn(b, r); off = 120.f; }
+    else { num = __fsub_rn(r, g); off = 240.f; }
+    if (!scalar_tail) {                                   // vector loop: the +360 of a negative V == R hue is inside the FMA
+        if (r == v && num < 0.f) off = 360.f;
+        h = __fmaf_rn(num, __fdiv_rn(60.f, dd), off);
+    } else {                                              // scalar loop: 60 / x in double, +360 afterwards
+        h = __fmaf_rn(num, __double2float_rn(__ddiv_rn(60.0, (double)dd)), off);
+        if (h < 0.f) h = __fadd_rn(h, 360.f);
+    }
+}
+
+__device__ __forceinline__ void hsv_to_bgr(float h, float s, float v, float& b, float& g, float& r) {
+    const float hs = __fmul_rn(h, 6.f / 360.f);
+    const float pre = truncf(hs);
+    const float f = __fsub_rn(hs, pre);
+    int sector = (int)pre - 6 * (int)truncf(__fmul_rn(pre, 1.f / 6.f));
+    if (sector < 0) sector += 6;
+    const float t0 = v;
+    const float t1 = __fmul_rn(v, __fsub_rn(1.f, s));
+    const float t2 = __fmul_rn(v, __fmaf_rn(-s, f, 1.f));
+    const float t3 = __fmul_rn(v, __fmaf_rn(-s, __fsub_rn(1.f, f), 1.f));
+    switch (sector) {                                     // cv2's sector table {1,3,0} {1,0,2} {3,0,1} {0,2,1} {0,1,3} {2,1,0}
+        case 0: b = t1; g = t3; r = t0; break;
+        case 1: b = t1; g = t0; r = t2; break;
+        case 2: b = t3; g = t0; r = t1; break;
+        case 3: b = t0; g = t2; r = t1; break;
+        case 4: b = t0; g = t1; r = t3; break;
+        default: b = t2; g = t1; r = t0; break;
+    }
+}
+
+// numpy's float32 -> uint8 cast on x86: truncate toward zero, keep the low 8 bits (290.3 -> 34, -5.7 -> 251)
+__device__ __forceinline__ unsigned char to_u8_wrap(float x) { return (unsigned char)__float2int_rz(x); }
+
+// grid (blocks per image, B): block x strides over the rows of image blockIdx.y, the threads over the pixels of a row
+__global__ void __launch_bounds__(256) photometric_distort_kernel(const unsigned char* const* __restrict__ src,
+                                                                  const int* __restrict__ src_wh,
+                                                                  const long long* __restrict__ src_pitch,
+                                                                  const mdb_photometric_params* __restrict__ params,
+                                                                  unsigned char* const* __restrict__ dst,
+                                                                  const long long* __restrict__ dst_pitch) {
+    const int b = blockIdx.y;
+    const int W = src_wh[2 * b], H = src_wh[2 * b + 1];
+    const mdb_photometric_params p = params[b];
+    if (W <= 0 || H <= 0 || (unsigned)p.perm > 5u || (unsigned)p.contrast_last > 1u) return;
+    const int tail0 = W - W % kHsvSimdWidth;
+    for (int y = blockIdx.x; y < H; y += gridDim.x) {
+        const unsigned char* s_row = src[b] + (long long)y * src_pitch[b];
+        unsigned char* d_row = dst[b] + (long long)y * dst_pitch[b];
+        for (int x = threadIdx.x; x < W; x += blockDim.x) {
+            float c[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                c[k] = __fadd_rn((float)s_row[3 * x + k], p.brightness);
+                if (!p.contrast_last) c[k] = __fmul_rn(c[k], p.contrast);
+            }
+            float h, s, v;
+            bgr_to_hsv(c[0], c[1], c[2], x >= tail0, h, s, v);
+            s = __fmul_rn(s, p.saturation);
+            h = __fadd_rn(h, p.hue);
+            if (h > 360.f) h = __fsub_rn(h, 360.f);
+            if (h < 0.f) h = __fadd_rn(h, 360.f);
+            hsv_to_bgr(h, s, v, c[0], c[1], c[2]);
+            if (p.contrast_last) {
+#pragma unroll
+                for (int k = 0; k < 3; ++k) c[k] = __fmul_rn(c[k], p.contrast);
+            }
+            float o0 = c[0], o1 = c[1], o2 = c[2];       // pd.py:143-145 perms: out[k] = c[perm[k]]
+            switch (p.perm) {
+                case 1: o1 = c[2]; o2 = c[1]; break;
+                case 2: o0 = c[1]; o1 = c[0]; break;
+                case 3: o0 = c[1]; o1 = c[2]; o2 = c[0]; break;
+                case 4: o0 = c[2]; o1 = c[0]; o2 = c[1]; break;
+                case 5: o0 = c[2]; o2 = c[0]; break;
+                default: break;
+            }
+            d_row[3 * x] = to_u8_wrap(o0);
+            d_row[3 * x + 1] = to_u8_wrap(o1);
+            d_row[3 * x + 2] = to_u8_wrap(o2);
+        }
+    }
+}
+
 }  // namespace
+
+extern "C" int mdb_photometric_distort_u8(const unsigned char* const* src, const int* src_wh, const long long* src_pitch,
+                                          const mdb_photometric_params* params, unsigned char* const* dst,
+                                          const long long* dst_pitch, int B, void* stream) {
+    if (!src || !src_wh || !src_pitch || !params || !dst || !dst_pitch) return MDB_EINVAL;
+    if (B <= 0 || B > 65535) return MDB_EINVAL;
+    const int per_image = mdb::num_sms() * 8 / B;
+    dim3 grid(per_image < 1 ? 1 : per_image, B);
+    photometric_distort_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, src_wh, src_pitch, params, dst, dst_pitch);
+    return (int)cudaGetLastError();
+}
 
 extern "C" int mdb_warp_affine_normalize_u8(const unsigned char* const* src, const int* src_wh, const long long* src_pitch,
                                             const double* trans_inv, const unsigned char* flip, int B, int out_w, int out_h,

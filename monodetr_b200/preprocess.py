@@ -4,11 +4,16 @@
   get_affine_transform(center, scale, rot, output_size, shift, inv)   lib/datasets/kitti/kitti_utils.py:347-381 (host: 6 numbers
                                                                       per image; cv2.getAffineTransform restated as a 3-point solve)
   ImageBatchPreprocessor(resolution, mean, std)(images_u8, trans_inv, flip)  -> (B, 3, H, W) fp32 normalised, on the device
+  PhotometricDistort().sample()                                       lib/datasets/kitti/pd.py:376-397 (`aug_pd`): the host draws
+  ImageBatchPreprocessor(...)(images_u8, trans_inv, flip, distort=[records])  the distortion on the device first (a second launch,
+                                                                      csrc/preprocess.cu), bit-identical to pd.py + cv2 + numpy
 
 `images_u8`: list of (H_i, W_i, 3) uint8 tensors (ragged, as decoded; CPU tensors are uploaded through pinned memory, CUDA tensors
 are used in place).  The result is bit-identical to PIL's AFFINE/BILINEAR transform followed by the reference's numpy
 normalisation (tests/test_preprocess_gpu.py, tests/golden/preprocess.npz).
 """
+from typing import NamedTuple
+
 import numpy as np
 import torch
 
@@ -60,6 +65,82 @@ def get_affine_transform(center, scale, rot, output_size, shift=np.array([0, 0],
     return trans
 
 
+class PhotometricParams(NamedTuple):
+    """One image's draws of the reference's PhotometricDistort (the C record mdb_photometric_params).  A step whose coin said no
+    carries its neutral value, which gives the same bits as skipping it."""
+    brightness: float = 0.0         # RandomBrightness delta
+    contrast: float = 1.0           # RandomContrast alpha
+    saturation: float = 1.0         # RandomSaturation factor
+    hue: float = 0.0                # RandomHue delta (degrees)
+    contrast_last: int = 0          # 0: contrast before the HSV steps (pd[:-1]); 1: after them (pd[1:])
+    perm: int = 0                   # RandomLightingNoise: index into pd.py's perms (0 = identity)
+
+
+class PhotometricDistort:
+    """lib/datasets/kitti/pd.py:376-397 split in two: `sample()` makes the reference's random draws on the host, and
+    ImageBatchPreprocessor(..., distort=[records]) applies them to the whole batch on the device.  In the dataset,
+    `pd_params = self.pd.sample()` replaces the three lines of kitti_dataset.py:136-138."""
+
+    def __init__(self, brightness_delta=32, contrast=(0.5, 1.5), saturation=(0.5, 1.5), hue_delta=18.0):
+        self.brightness_delta = brightness_delta        # pd.py:185-188, 170-175, 114-119, 128-131 defaults
+        self.contrast = contrast
+        self.saturation = saturation
+        self.hue_delta = hue_delta
+
+    def sample(self, rs=np.random):
+        """The same `randint` / `uniform` calls as PhotometricDistort.__call__, in the same order and on the same generator (the
+        global numpy.random unless `rs` is given), including the ones whose step is then skipped; so the flip and crop draws that
+        follow in __getitem__ see the stream they see in the reference."""
+        p = {}
+        if rs.randint(2):
+            p["brightness"] = rs.uniform(-self.brightness_delta, self.brightness_delta)
+        contrast_first = rs.randint(2)
+        p["contrast_last"] = 0 if contrast_first else 1
+        if contrast_first and rs.randint(2):
+            p["contrast"] = rs.uniform(*self.contrast)
+        if rs.randint(2):
+            p["saturation"] = rs.uniform(*self.saturation)
+        if rs.randint(2):
+            p["hue"] = rs.uniform(-self.hue_delta, self.hue_delta)
+        if not contrast_first and rs.randint(2):
+            p["contrast"] = rs.uniform(*self.contrast)
+        if rs.randint(2):
+            p["perm"] = rs.randint(6)
+        return PhotometricParams(**p)
+
+
+_RECORD_DTYPE = np.dtype([("brightness", "<f4"), ("contrast", "<f4"), ("saturation", "<f4"), ("hue", "<f4"),
+                          ("contrast_last", "<i4"), ("perm", "<i4")])         # 24 bytes, include/monodetr_b200.h
+
+
+def pack_photometric(records, B):
+    """(B, 6) records -> the bytes of B mdb_photometric_params (4 float32, 2 int32 each); ValueError on a malformed record."""
+    if len(records) != B:
+        raise ValueError(f"distort: {len(records)} records for {B} images")
+    out = np.zeros(B, dtype=_RECORD_DTYPE)
+    for i, r in enumerate(records):
+        try:
+            if len(r) != len(PhotometricParams._fields):
+                raise ValueError(f"{len(r)} fields")
+            r = PhotometricParams(*r)
+            vals = np.array(r[:4], np.float64)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"distort[{i}]: not a record of 6 numbers ({e})") from None
+        if not np.isfinite(vals).all() or np.any(np.abs(vals) > np.finfo(np.float32).max):
+            raise ValueError(f"distort[{i}]: non-finite or out-of-range value {r}")
+        if r.contrast_last not in (0, 1) or int(r.contrast_last) != r.contrast_last:
+            raise ValueError(f"distort[{i}]: contrast_last must be 0 or 1, got {r.contrast_last!r}")
+        if r.perm not in range(6) or int(r.perm) != r.perm:
+            raise ValueError(f"distort[{i}]: perm must be in 0..5, got {r.perm!r}")
+        out[i] = (*vals.astype(np.float32), int(r.contrast_last), int(r.perm))
+    return out
+
+
+def _require_cuda(device):
+    if device.type != "cuda":
+        raise RuntimeError("ImageBatchPreprocessor: a CUDA device is required (there is no CPU path)")
+
+
 class ImageBatchPreprocessor:
     def __init__(self, resolution=(1280, 384), mean=KITTI_MEAN, std=KITTI_STD, device="cuda"):
         self.resolution = (int(resolution[0]), int(resolution[1]))        # (W, H) as the reference's `resolution`
@@ -67,11 +148,69 @@ class ImageBatchPreprocessor:
         self.std = np.asarray(std, np.float32)
         self.device = torch.device(device)
 
-    def __call__(self, images, trans_inv, flip=None):
-        """images: list of (H, W, 3) uint8 tensors; trans_inv: (B, 2, 3) array (PIL `data`); flip: optional (B,) bools."""
+    def __call__(self, images, trans_inv, flip=None, distort=None):
+        """images: list of (H, W, 3) uint8 tensors; trans_inv: (B, 2, 3) array (PIL `data`); flip: optional (B,) bools;
+        distort: optional list of B PhotometricParams (PhotometricDistort.sample()), applied to each source image before the flip
+        and the warp, as the reference's `aug_pd`.  The images themselves are never modified."""
         B = len(images)
-        if self.device.type != "cuda":
-            raise RuntimeError("ImageBatchPreprocessor: a CUDA device is required (there is no CPU path)")
+        _require_cuda(self.device)
+        records = None if distort is None else pack_photometric(distort, B)
+        dev_imgs = self._device_images(images)
+        # ONE pinned upload for all per-image metadata: pointers | pitches | matrices (fp64) | (W, H) int32 pairs | flip flags
+        # [| distorted-image pointers | their pitches | distortion records]
+        n_base = B * 9 + (B + 7) // 8
+        buf = np.zeros(n_base + (0 if records is None else 5 * B), np.int64)
+        for i, im in enumerate(dev_imgs):
+            buf[i], buf[B + i] = im.data_ptr(), im.stride(0)
+        buf[2 * B:8 * B].view(np.float64)[:] = np.asarray(trans_inv, np.float64).reshape(B * 6)
+        wh = buf[8 * B:9 * B].view(np.int32)
+        wh[0::2], wh[1::2] = [im.shape[1] for im in dev_imgs], [im.shape[0] for im in dev_imgs]
+        if flip is not None:
+            buf[9 * B:n_base].view(np.uint8)[:B] = np.asarray(flip).astype(np.uint8)
+        scratch = None
+        if records is not None:
+            # one flat buffer holds every distorted image, rows packed (pitch 3 * W)
+            sizes = [im.shape[0] * im.shape[1] * 3 for im in dev_imgs]
+            scratch = torch.empty(max(sum(sizes), 1), dtype=torch.uint8, device=self.device)
+            offs = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64)
+            buf[n_base:n_base + B] = scratch.data_ptr() + offs
+            buf[n_base + B:n_base + 2 * B] = [3 * im.shape[1] for im in dev_imgs]
+            buf[n_base + 2 * B:n_base + 5 * B].view(_RECORD_DTYPE)[:] = records
+        meta = torch.from_numpy(buf).pin_memory().to(self.device, non_blocking=True)
+        base = meta.data_ptr()
+        ptrs, pitch, trd, whd, fld = base, base + 8 * B, base + 16 * B, base + 64 * B, base + 72 * B
+        W, H = self.resolution
+        out = torch.empty(B, 3, H, W, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            if records is not None:
+                dptrs, dpitch, recd = base + 8 * n_base, base + 8 * (n_base + B), base + 8 * (n_base + 2 * B)
+                _lib.call("mdb_photometric_distort_u8", ptrs, whd, pitch, recd, dptrs, dpitch, B)
+                ptrs, pitch = dptrs, dpitch                     # the warp samples the distorted images
+            _lib.call("mdb_warp_affine_normalize_u8", ptrs, whd, pitch, trd, fld, B, W, H, self.mean.ctypes.data, self.std.ctypes.data,
+                      out)
+        return out
+
+    def distort(self, images, distort):
+        """The distortion alone: list of (H, W, 3) uint8 tensors + B records -> list of distorted (H, W, 3) uint8 CUDA tensors,
+        bit-identical to the reference's `pd(img.astype(np.float32)).astype(np.uint8)` (kitti_dataset.py:136-138)."""
+        B = len(images)
+        _require_cuda(self.device)
+        records = pack_photometric(distort, B)
+        dev_imgs = self._device_images(images)
+        outs = [torch.empty(tuple(im.shape), dtype=torch.uint8, device=self.device) for im in dev_imgs]
+        buf = np.zeros(8 * B, np.int64)                 # src pointers | src pitches | (W, H) | dst pointers | dst pitches | records
+        for i, (im, o) in enumerate(zip(dev_imgs, outs)):
+            buf[i], buf[B + i], buf[3 * B + i], buf[4 * B + i] = im.data_ptr(), im.stride(0), o.data_ptr(), o.stride(0)
+        wh = buf[2 * B:3 * B].view(np.int32)
+        wh[0::2], wh[1::2] = [im.shape[1] for im in dev_imgs], [im.shape[0] for im in dev_imgs]
+        buf[5 * B:8 * B].view(_RECORD_DTYPE)[:] = records
+        meta = torch.from_numpy(buf).pin_memory().to(self.device, non_blocking=True)
+        base = meta.data_ptr()
+        with torch.cuda.device(self.device):
+            _lib.call("mdb_photometric_distort_u8", base, base + 16 * B, base + 8 * B, base + 40 * B, base + 24 * B, base + 32 * B, B)
+        return outs
+
+    def _device_images(self, images):
         dev_imgs = []
         for im in images:
             if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3:
@@ -81,21 +220,4 @@ class ImageBatchPreprocessor:
             if im.stride(2) != 1 or im.stride(1) != 3:
                 im = im.contiguous()
             dev_imgs.append(im)
-        # ONE pinned upload for all per-image metadata: pointers | pitches | matrices (fp64) | (W, H) int32 pairs | flip flags
-        buf = np.zeros(B * 9 + (B + 7) // 8, np.int64)
-        for i, im in enumerate(dev_imgs):
-            buf[i], buf[B + i] = im.data_ptr(), im.stride(0)
-        buf[2 * B:8 * B].view(np.float64)[:] = np.asarray(trans_inv, np.float64).reshape(B * 6)
-        wh = buf[8 * B:9 * B].view(np.int32)
-        wh[0::2], wh[1::2] = [im.shape[1] for im in dev_imgs], [im.shape[0] for im in dev_imgs]
-        if flip is not None:
-            buf[9 * B:].view(np.uint8)[:B] = np.asarray(flip).astype(np.uint8)
-        meta = torch.from_numpy(buf).pin_memory().to(self.device, non_blocking=True)
-        base = meta.data_ptr()
-        ptrs, pitch, trd, whd, fld = base, base + 8 * B, base + 16 * B, base + 64 * B, base + 72 * B
-        W, H = self.resolution
-        out = torch.empty(B, 3, H, W, dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.call("mdb_warp_affine_normalize_u8", ptrs, whd, pitch, trd, fld, B, W, H, self.mean.ctypes.data, self.std.ctypes.data,
-                      out)
-        return out
+        return dev_imgs
