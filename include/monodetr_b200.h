@@ -111,10 +111,15 @@ int mdb_msda_fused_backward_f32(const float* value, const int64_t* spatial_shape
  * with B=1, H=1, W=M, Cin=K, Cout=N, kh=kw=1, stride=1, pad=0 (w itself is already "packed").
  * Supported: kh=kw in {1,3}, stride in {1,2}, Cin%4==0, 16-byte aligned pointers; Cout%4==0 for dgrad / wgrad (the
  * forward writes any Cout, e.g. the 3-class / 81-bin head widths of monodetr.py:102-117); outputs below 2^31 elements.
- * Results do not depend on the batch size (same image -> same bits) and are bit-reproducible run to run for
- * forward / dgrad; wgrad accumulates its split-K partial sums with fp32 atomics.  The one forward shape with
- * >= 256 k-blocks and few tiles (3x3 stride-2 2048->256, monodetr.py:83-91) reduces through the scratch buffer the caller
- * registers with mdb_set_workspace (per device; the library itself never allocates or frees device memory).
+ * Forward and dgrad are bit-reproducible run to run, and image b of a batch gets the same bits as the same image in any
+ * other batch, in every precision mode.  wgrad accumulates its split-K partial sums with fp32 atomics.  A forward with
+ * >= 256 k-blocks of 32 input channels (kh*kw*ceil(Cin/32); the 3x3 stride-2 2048->256 of monodetr.py:83-91), Cout > 64,
+ * Cout % 4 == 0, no residual, no ReLU, a NULL or 16-byte aligned bias and precision mode 1 or 2 is split into
+ * ceil(k-blocks/32) slices whatever the batch; the slices go through the scratch buffer the caller registers with
+ * mdb_set_workspace (per device; the library itself never allocates or frees device memory) and are added in slice order.
+ * The one exception to batch independence: when B*Ho*Wo*Cout*slices >= 2^31 that forward runs unsplit, so its bits match
+ * a smaller batch's only while the product stays below 2^31 (below 3884 images for the 12x40 neck conv).
+ * Below that bound mdb_conv2d_forward_workspace_bytes is B times a per-image size.
  */
 /* Arithmetic of the tensor-core family (a process-wide numerical setting): 2 (default) = error-compensated BF16x3 (operands
  * split into bf16 hi + lo, A_hi*B_hi + A_lo*B_hi + A_hi*B_lo at twice the TF32 tensor rate, dropped terms ~2^-17 per product;
@@ -181,6 +186,9 @@ int mdb_colsum_f32(const float* x, float* out, long long M, int N, int accumulat
  * bytes (nonzero = ignore) or NULL.  lse [B][H][Lq] is written by forward and read by backward.
  * Dropout on the probabilities: drop_p in [0,1); *seed is read on the device (CUDA-graph safe); `site`
  * decorrelates call sites.  delta_ws: B*H*Lq floats of workspace.
+ * A query row whose keys are all masked gets out = 0 and lse = -inf, and contributes nothing to the backward: its dq row
+ * is 0 and it adds nothing to dk / dv (a batch whose keys are all masked gets dq = dk = dv = 0).  torch's
+ * F.multi_head_attention_forward returns NaN for such a row instead.
  */
 int mdb_attention_forward_f32(const float* q, const float* k, const float* v, const unsigned char* key_padding_mask,
                               float* out, float* lse, int B, int H, int Lq, int Lk, int head_dim,

@@ -562,12 +562,15 @@ int mdb_get_precision(void) { return g_precision; }
 
 namespace {
 
-// Split-K decision of the forward (shared by the launcher and mdb_conv2d_forward_workspace_bytes): a handful of tiles
-// with a very long reduction (the 3x3 stride-2 2048->256 neck convolution: 16-32 tiles x 576 k-blocks kept a fifth of
-// the SMs busy for 0.3 ms).  Returns the number of slices (0 = no split-K).
-int forward_splitk_slices(int precision, int tiles, int kblocks, int bn, bool plain_epilogue, int Cout, long long out_elems) {
+// Split-K decision of the forward (shared by the launcher and mdb_conv2d_forward_workspace_bytes) for very long
+// reductions (the 3x3 stride-2 2048->256 neck convolution: 16-32 tiles x 576 k-blocks kept a fifth of the SMs busy for
+// 0.3 ms).  Returns the number of slices (0 = no split-K).  The decision deliberately ignores the tile count, which grows
+// with the batch: it depends on the reduction length, Cout, the epilogue and (in the caller) the bias alignment, so an
+// image is summed in the same order whatever batch it is in.  The one batch-dependent term is the 32-bit bound on the
+// scratch size below.
+int forward_splitk_slices(int precision, int kblocks, int bn, bool plain_epilogue, int Cout, long long out_elems) {
     const int kb_per_slice = 32;
-    if (precision == 0 || bn != 128 || tiles * 2 > num_sms() || kblocks < 256 || !plain_epilogue || Cout % 4) return 0;
+    if (precision == 0 || bn != 128 || kblocks < 256 || !plain_epilogue || Cout % 4) return 0;
     const int slices = (kblocks + kb_per_slice - 1) / kb_per_slice;
     return (out_elems * slices < (1ll << 31)) ? slices : 0;
 }
@@ -613,7 +616,7 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
     dim3 grid((Cout + bn - 1) / bn, n_groups * p.tiles_x * p.tiles_y, 1);
     const long long out_elems = (long long)B * g.Ho * g.Wo * Cout;
     const int slices = ((reinterpret_cast<uintptr_t>(bias) & 15u) == 0)
-                           ? forward_splitk_slices(precision, (int)(grid.x * grid.y), p.ntaps * p.cblocks, bn, !residual && !p.relu, Cout, out_elems)
+                           ? forward_splitk_slices(precision, p.ntaps * p.cblocks, bn, !residual && !p.relu, Cout, out_elems)
                            : 0;
     if (query_ws) {
         *query_ws = sizeof(float) * (size_t)out_elems * slices;
@@ -645,8 +648,9 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
         if (rc) return rc;
     }
     // Split-K (see forward_splitk_slices): slices write partial tiles to the caller's scratch buffer and a second kernel adds
-    // them in a fixed order (+ bias): bit-reproducible, unlike atomic accumulation.  The slice length is fixed and only
-    // reductions >= 256 k-blocks take this path, so the summation order does not depend on the batch size.
+    // them in a fixed order (+ bias): bit-reproducible, unlike atomic accumulation.  Whether a shape splits and into how
+    // many slices of a fixed length depends on the per-image problem only (up to the scratch bound in
+    // forward_splitk_slices), so the summation order of an image does not depend on the batch size.
     {
         if (slices > 0) {
             float* ws = nullptr;

@@ -251,7 +251,8 @@ def conv2d_wgrad(dy, x, rowscale=None, kh=1, kw=1, stride=1, pad=0, with_bias_gr
 
 # ---- linear layers = 1x1 convolution over a 1-row "image" of M pixels ---------------------------------
 def set_precision(mode: str):
-    """'bf16x3' (default: error-compensated BF16 for forward / dgrad with weights split once per step, 3xTF32 wgrad),
+    """'bf16x3' (default: error-compensated BF16 for forward / dgrad with weights split once per step, and for wgrad with both
+    operands split in the kernel),
     'tf32x3' (error-compensated TF32 everywhere, ~fp32 accuracy) or 'tf32' (single pass, operands rounded to nearest)."""
     _lib.check(_lib.lib().mdb_set_precision({"tf32": 0, "tf32x3": 1, "bf16x3": 2}[mode]), "set_precision")
 
