@@ -111,6 +111,9 @@ int mdb_msda_fused_backward_f32(const float* value, const int64_t* spatial_shape
  * with B=1, H=1, W=M, Cin=K, Cout=N, kh=kw=1, stride=1, pad=0 (w itself is already "packed").
  * Supported: kh=kw in {1,3}, stride in {1,2}, Cin%4==0, 16-byte aligned pointers; Cout%4==0 for dgrad / wgrad (the
  * forward writes any Cout, e.g. the 3-class / 81-bin head widths of monodetr.py:102-117); outputs below 2^31 elements.
+ * Forward and dgrad store their output with TMA (staged in shared memory, residual or mask fetched by TMA) when the output
+ * width is a multiple of 4 and y / dx, residual and relu_mask are 16-byte aligned, and from registers otherwise (e.g. the
+ * odd head widths); both give the same bits.
  * Forward and dgrad are bit-reproducible run to run, and image b of a batch gets the same bits as the same image in any
  * other batch, in every precision mode.  wgrad accumulates its split-K partial sums with fp32 atomics.  A forward with
  * >= 256 k-blocks of 32 input channels (kh*kw*ceil(Cin/32); the 3x3 stride-2 2048->256 of monodetr.py:83-91), Cout > 64,

@@ -13,8 +13,9 @@
 // Layouts: activations NHWC fp32 [B][H][W][C]; packed weights [tap][Cout][Cin]; output NHWC.
 // Tile: 128 output pixels (tw x th pixels of tb consecutive images) x BN output channels, K step = 32 fp32
 // (one 128-byte swizzle span).  Persistent CTAs (one per SM) walk the tiles.  Warp roles: warps 0-7 = two consumer
-// warpgroups (64 rows each: operand staging, wgmma, fused epilogue straight from the accumulator registers), warp 8 =
-// TMA producer.  smem ring of STAGES stages, mbarrier full/empty pairs.
+// warpgroups (64 rows each: operand staging, wgmma, fused epilogue -- through a shared-memory staging tile and TMA
+// stores for fprop / dgrad, straight from the accumulator registers otherwise), warp 8 = TMA producer.  smem ring of
+// STAGES stages, mbarrier full/empty pairs.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -56,6 +57,9 @@ struct TcParams {
     int Mo_rows;                     // wgrad: number of valid output rows (Cout)
     int No, ldo;
     int relu, atomic_out, round_out;   // round_out: store round-to-nearest TF32 (next consumer is a tensor-core operand)
+    // TMA epilogue (mapO / mapR): 0 = register epilogue.  epi_load: 1 = residual, 2 = ReLU mask fetched by TMA through mapR
+    // into the staging tile.  Warpgroup 1's box starts half_{x,y,b} pixels / rows / images after warpgroup 0's.
+    int epi_tma, epi_load, half_x, half_y, half_b;
     const float* bias;               // [No] or null
     const float* residual;           // same indexing as out, or null
     const float* relu_mask;          // same indexing as out: out *= (mask > 0), or null
@@ -73,6 +77,20 @@ __device__ __forceinline__ uint32_t raw_off(int row, int k) {
 
 __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
+// Shared memory of one kernel instance: the TMA ring, the epilogue staging tile of fprop / dgrad (two warpgroups x 64 rows
+// x BN fp32, as 32-channel boxes of 64 128-byte swizzled rows) when it fits beside the ring, the consumers' B operand
+// tile(s), barriers.
+template <int BN, int STAGES, int MODE, int PREC>
+struct TcSmem {
+    static constexpr bool kConvB = !(PREC == 2 && MODE == 0);
+    static constexpr int kRing = STAGES * (kTileABytes + BN * 128);
+    static constexpr int kStage = 2 * 64 * BN * 4;
+    static constexpr int kConv = kConvB ? (PREC == 1 ? 2 : 1) * BN * 128 : 0;
+    static constexpr int kFixed = kRing + kConv + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr bool kTmaEpi = MODE == 0 && kFixed + kStage <= 227 * 1024;
+    static constexpr int kBytes = kFixed + (kTmaEpi ? kStage : 0);
+};
+
 // Persistent, warp-specialised kernel.  Each CTA walks tiles  tile = blockIdx.x + i * gridDim.x.
 //   warp 8          TMA producer (smem ring of STAGES stages, full/empty mbarriers)
 //   warps 0-7       two consumer warpgroups; warpgroup g owns rows [64g, 64g+64) of the 128-row tile.  Per k-block each
@@ -89,6 +107,7 @@ __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__
 template <int BN, int STAGES, int MODE /*0 fprop/dgrad, 1 wgrad*/, bool B_MN, int PREC>
 __global__ void __launch_bounds__(kThreadsTC, 1)
 tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                    const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapR,
                     const __grid_constant__ TcParams p) {
     constexpr bool A_MN = (MODE == 1);
     static_assert(!(MODE == 1) || B_MN, "wgrad reads both operands MN-major");
@@ -98,13 +117,15 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     constexpr bool CONVB = !BF_B;                                 // consumers rewrite B into the operand tile(s)
     constexpr int kTileBBytes = BN * 128;
     constexpr int kRawBytes = kTileABytes + kTileBBytes;          // what TMA delivers per stage
-    constexpr int kConvBytes = CONVB ? (PREC == 1 ? 2 : 1) * kTileBBytes : 0;
+    using SM = TcSmem<BN, STAGES, MODE, PREC>;
     constexpr int NACC = BN / 2;
 
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint8_t* bconv = smem + STAGES * kRawBytes;                   // [hi | lo] operand tiles of the current k-block (CONVB)
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(bconv + kConvBytes);
+    uint8_t* stage_out = smem + STAGES * kRawBytes;               // epilogue staging tile (SM::kTmaEpi)
+    uint8_t* bconv = stage_out + (SM::kTmaEpi ? SM::kStage : 0);  // [hi | lo] operand tiles of the current k-block (CONVB)
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(bconv + SM::kConv);
     uint64_t* empty_bar = full_bar + STAGES;
+    uint64_t* epi_bar = empty_bar + STAGES;                       // per warpgroup: its residual / mask box has landed
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -146,10 +167,16 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
         if (smem_u32(smem) & 1023u) __trap();                     // SWIZZLE_128B tiles need 1024-byte aligned stages
         tma_prefetch_desc(&mapA);
         tma_prefetch_desc(&mapB);
+        if (SM::kTmaEpi && p.epi_tma) {
+            tma_prefetch_desc(&mapO);
+            if (p.epi_load) tma_prefetch_desc(&mapR);
+        }
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], kConsumerThreads / 32);      // one arrival per consumer warp
         }
+        mbar_init(&epi_bar[0], 1);
+        mbar_init(&epi_bar[1], 1);
         fence_mbar_init();
     }
     __syncthreads();
@@ -218,10 +245,26 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     const int g = lane >> 2, tig = lane & 3;
     const int r0 = wg * 64 + (warp & 3) * 16 + g;                 // this thread's tile rows: r0 and r0 + 8
     const int ctid = threadIdx.x;                                 // 0..255
+    // TMA epilogue: warpgroup wg stages its 64 x BN results in its half of stage_out and thread 128 * wg (the leader, which
+    // owns the warpgroup's bulk groups) stores them; the warpgroup goes on to the next tile while the store drains.
+    const bool epi_tma = SM::kTmaEpi && p.epi_tma;
+    const bool leader = (ctid & 127) == 0;
+    uint8_t* my_stage = stage_out + wg * (SM::kStage / 2);
+    uint32_t epi_phase = 0;
     int git = 0;
     for (int tix = blockIdx.x; tix < p.total_tiles; tix += gridDim.x) {
         const Tile t = decode(tix);
         if (p.atomic_out && t.iters == 0) continue;              // nothing to add
+        // origin of this warpgroup's box: channel, then pixel x / y / image / split-K slice
+        const int c1 = t.x0 + wg * p.half_x, c2 = t.y0 + wg * p.half_y, c3 = t.img + wg * p.half_b, c4 = t.slice;
+        if (epi_tma && p.epi_load && leader) {
+            // the previous tile's store has read the staging tile: fetch this tile's residual / mask into it now, while
+            // the k-blocks run
+            bulk_wait_read_all();
+            mbar_arrive_expect_tx(&epi_bar[wg], SM::kStage / 2);
+#pragma unroll
+            for (int c = 0; c < BN / 32; ++c) tma_load_5d(my_stage + c * 8192, &mapR, &epi_bar[wg], t.n0 + 32 * c, c1, c2, c3, c4);
+        }
         float acc[NACC];
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
@@ -348,6 +391,56 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
             if (lane == 0) mbar_arrive(&empty_bar[s]);            // this warp is done with the stage
         }
 
+        if (epi_tma) {
+            // ---- TMA epilogue: the same operations in the same order as the register epilogue below, through the
+            // staging tile (which holds the TMA-fetched residual or mask, read in place); the map clips the box at the
+            // output's bounds, so rows and channels past them are computed but never stored.
+            if (p.epi_load) {
+                mbar_wait(&epi_bar[wg], epi_phase);
+                epi_phase ^= 1;
+            } else {
+                if (leader) bulk_wait_read_all();
+                named_bar_sync(2 + wg, 128);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = r0 + h * 8, rr = row - 64 * wg;
+                const float* gmask = nullptr;                     // mask beside a TMA-fetched residual: read from global
+                if (p.relu_mask && p.epi_load != 2) {
+                    const int lyt = row / p.tw, lx = row - lyt * p.tw;
+                    const int ib = lyt / p.th, ly = lyt - ib * p.th;
+                    const int y = t.y0 + ly, x = t.x0 + lx, img = t.img + ib;
+                    if ((y < p.Ho) && (x < p.Wo) && (img < p.n_img))
+                        gmask = p.relu_mask + (size_t)((img * p.out_H + y * p.out_sy + p.out_oy) * p.out_W + x * p.out_sx + p.out_ox) * p.ldo;
+                }
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int n = t.n0 + j * 8 + tig * 2;         // No % 4 == 0: n < No implies n + 1 < No
+                    if (n >= p.No) continue;
+                    float2* sp = reinterpret_cast<float2*>(my_stage + (j >> 2) * 8192 + raw_off<false>(rr, (j & 3) * 8 + tig * 2));
+                    float v[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};   // (the register path's * 1.f: exact)
+                    if (p.bias) { v[0] += p.bias[n]; v[1] += p.bias[n + 1]; }
+                    if (p.epi_load == 1) { const float2 e = *sp; v[0] += e.x; v[1] += e.y; }
+                    if (p.relu) { v[0] = fmaxf(v[0], 0.f); v[1] = fmaxf(v[1], 0.f); }
+                    if (p.relu_mask) {
+                        float2 m = make_float2(0.f, 0.f);
+                        if (p.epi_load == 2) m = *sp;
+                        else if (gmask) m = *reinterpret_cast<const float2*>(gmask + n);
+                        v[0] = m.x > 0.f ? v[0] : 0.f; v[1] = m.y > 0.f ? v[1] : 0.f;
+                    }
+                    if (p.round_out) { v[0] = round_tf32(v[0]); v[1] = round_tf32(v[1]); }
+                    *sp = make_float2(v[0], v[1]);
+                }
+            }
+            fence_proxy_async_smem();      // generic-proxy writes -> visible to the bulk copy's async-proxy reads
+            named_bar_sync(2 + wg, 128);
+            if (leader) {
+#pragma unroll
+                for (int c = 0; c < BN / 32; ++c) tma_store_5d(&mapO, my_stage + c * 8192, t.n0 + 32 * c, c1, c2, c3, c4);
+                bulk_commit();
+            }
+            continue;
+        }
         // ---- epilogue: accumulator registers -> fused bias / residual / ReLU / mask / row-scale -> global ------------
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -412,6 +505,8 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
             }
         }
     }
+    // The grid's completion (which a programmatic dependent waits for) must imply that its bulk stores have landed.
+    if (epi_tma && leader) bulk_wait_all();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -439,12 +534,14 @@ int current_device() {
 
 // `grid` carries the logical tile counts (x = column tiles, y = row tiles, z = split-K slices); the kernel is
 // launched persistent with min(total_tiles, SMs) CTAs.
+// `o` / `r` describe the output and the residual or mask operand for the TMA epilogue (p.epi_tma); an instance whose ring
+// leaves no room for the staging tile runs the register epilogue whatever the launch asks.
 template <int BN, int STAGES, int MODE, bool B_MN, int PREC>
-int launch_tc(const CUtensorMap& a, const CUtensorMap& b, TcParams p, dim3 grid, cudaStream_t stream) {
-    constexpr bool convb = !(PREC == 2 && MODE == 0);
-    constexpr int smem = STAGES * (kTileABytes + BN * 128) + (convb ? (PREC == 1 ? 2 : 1) * BN * 128 : 0) +
-                         1024 /*align slack*/ + 256 /*barriers*/;
+int launch_tc(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r, TcParams p, dim3 grid,
+              cudaStream_t stream) {
+    constexpr int smem = TcSmem<BN, STAGES, MODE, PREC>::kBytes;
     static_assert(smem <= 227 * 1024, "dynamic shared memory budget");
+    if (!TcSmem<BN, STAGES, MODE, PREC>::kTmaEpi) p.epi_tma = p.epi_load = 0;
     auto kern = tc_conv_gemm_kernel<BN, STAGES, MODE, B_MN, PREC>;
     const cudaError_t e = set_max_dynamic_smem(kern, smem);
     if (e != cudaSuccess) return (int)e;
@@ -471,9 +568,9 @@ int launch_tc(const CUtensorMap& a, const CUtensorMap& b, TcParams p, dim3 grid,
         attr[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr;
         cfg.numAttrs = 1;
-        return (int)cudaLaunchKernelEx(&cfg, kern, a, b, p);
+        return (int)cudaLaunchKernelEx(&cfg, kern, a, b, o, r, p);
     }
-    kern<<<ctas, kThreadsTC, smem, stream>>>(a, b, p);
+    kern<<<ctas, kThreadsTC, smem, stream>>>(a, b, o, r, p);
     return (int)cudaGetLastError();
 }
 
@@ -527,11 +624,44 @@ void pick_tile3(int W, int H, int B, int n_pix, int* tw, int* th, int* tb) {
         }
 }
 
+bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) == 0; }
+
+// TMA epilogue of a fprop / dgrad launch (p.epi_tma).  The output -- and the residual, else the ReLU mask, which share its
+// indexing -- are 5-d tensor maps (C, W, H, B, split-K slice) over the launch's Wc x Hc x B pixel grid, starting `off`
+// elements into each buffer, with pixel strides sx, sy, sb elements; the box is one consumer warpgroup's 64 rows of the
+// tw x th x tb tile (the outermost tile dimension above 1 is halved).  Launches TMA cannot describe keep the register
+// epilogue: a channel count or row pitch that is not a multiple of 4 (16-byte pitches), or a buffer that is not 16-byte
+// aligned.
+int setup_epi_px(TcParams& p, CUtensorMap* mo, CUtensorMap* mr, size_t off, int Wc, int Hc, int B, uint64_t sx, uint64_t sy,
+                 uint64_t sb, int slices) {
+    p.epi_tma = p.epi_load = p.half_x = p.half_y = p.half_b = 0;
+    if (p.No % 4 || p.ldo % 4 || !aligned16(p.out + off) || (p.residual && !aligned16(p.residual + off)) ||
+        (p.relu_mask && !aligned16(p.relu_mask + off)))
+        return 0;
+    uint32_t box[5] = {32, (uint32_t)p.tw, (uint32_t)p.th, (uint32_t)p.tb, 1};
+    if (p.tb > 1) p.half_b = box[3] = p.tb / 2;
+    else if (p.th > 1) p.half_y = box[2] = p.th / 2;
+    else p.half_x = box[1] = p.tw / 2;
+    if (box[1] > 256 || box[2] > 256 || box[3] > 256) return 0;
+    uint64_t dims[5] = {(uint64_t)p.No, (uint64_t)Wc, (uint64_t)Hc, (uint64_t)B, (uint64_t)slices};
+    uint64_t str[5] = {1, sx, sy, sb, slices > 1 ? (uint64_t)p.slice_stride : sb * B};
+    int rc = make_map(mo, p.out + off, 5, dims, str, box, nullptr);
+    if (rc) return rc;
+    const float* opnd = p.residual ? p.residual : p.relu_mask;
+    if (opnd) {
+        rc = make_map(mr, opnd + off, 5, dims, str, box, nullptr);
+        if (rc) return rc;
+        p.epi_load = p.residual ? 1 : 2;
+    }
+    p.epi_tma = 1;
+    return 0;
+}
+
 // Launch the fprop / dgrad kernel (K-major B operand) for the arithmetic mode.
-int launch_fwd(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, dim3 grid, int bn, int precision, cudaStream_t stream) {
-    if (precision == 2) return bn == 64 ? launch_tc<64, 6, 0, false, 2>(ma, mb, p, grid, stream) : launch_tc<128, 5, 0, false, 2>(ma, mb, p, grid, stream);
-    if (precision == 1) return bn == 64 ? launch_tc<64, 5, 0, false, 1>(ma, mb, p, grid, stream) : launch_tc<128, 4, 0, false, 1>(ma, mb, p, grid, stream);
-    return bn == 64 ? launch_tc<64, 6, 0, false, 0>(ma, mb, p, grid, stream) : launch_tc<128, 5, 0, false, 0>(ma, mb, p, grid, stream);
+int launch_fwd(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr, const TcParams& p, dim3 grid, int bn, int precision, cudaStream_t stream) {
+    if (precision == 2) return bn == 64 ? launch_tc<64, 6, 0, false, 2>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 2>(ma, mb, mo, mr, p, grid, stream);
+    if (precision == 1) return bn == 64 ? launch_tc<64, 5, 0, false, 1>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 4, 0, false, 1>(ma, mb, mo, mr, p, grid, stream);
+    return bn == 64 ? launch_tc<64, 6, 0, false, 0>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 0>(ma, mb, mo, mr, p, grid, stream);
 }
 
 struct ConvGeom {
@@ -647,6 +777,10 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
         rc = make_map(&mb, w_packed, 3, dims, str, box, nullptr);
         if (rc) return rc;
     }
+    CUtensorMap mo, mr;   // TMA epilogue: y (or the split-K slices) and the residual, as (Cout, Wo, Ho, B, slice)
+    memset(&mo, 0, sizeof(mo));
+    memset(&mr, 0, sizeof(mr));
+    const uint64_t pix_x = (uint64_t)Cout, pix_y = pix_x * g.Wo, pix_b = pix_y * g.Ho;
     // Split-K (see forward_splitk_slices): slices write partial tiles to the caller's scratch buffer and a second kernel adds
     // them in a fixed order (+ bias): bit-reproducible, unlike atomic accumulation.  Whether a shape splits and into how
     // many slices of a fixed length depends on the per-image problem only (up to the scratch bound in
@@ -660,7 +794,9 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
             p.slice_stride = (int)out_elems;
             p.out = ws; p.bias = nullptr;
             grid.z = slices;
-            rc = launch_fwd(ma, mb, p, grid, 128, precision, stream);
+            rc = setup_epi_px(p, &mo, &mr, 0, g.Wo, g.Ho, B, pix_x, pix_y, pix_b, slices);
+            if (rc) return rc;
+            rc = launch_fwd(ma, mb, mo, mr, p, grid, 128, precision, stream);
             if (rc) return rc;
             const long long n4 = out_elems / 4;
             splitk_reduce_kernel<<<grid_cap(n4, 256, num_sms() * 8), 256, 0, stream>>>(
@@ -668,7 +804,9 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
             return (int)cudaGetLastError();
         }
     }
-    return launch_fwd(ma, mb, p, grid, bn, precision, stream);
+    rc = setup_epi_px(p, &mo, &mr, 0, g.Wo, g.Ho, B, pix_x, pix_y, pix_b, 1);
+    if (rc) return rc;
+    return launch_fwd(ma, mb, mo, mr, p, grid, bn, precision, stream);
 }
 
 // dx[B,H,W,Cin] = (conv_transpose(dy[B,Ho,Wo,Cout], w) + residual) * (relu_mask > 0);  w = fp32 packed [taps][Cout][Cin]
@@ -748,9 +886,15 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
             if (nt == 0) {   // no tap reaches this parity class (1x1 stride 2): result = (0 + residual) * mask
                 p.ntaps = 0;
             }
-            if (bf) rc = launch_fwd(ma, mb, p, grid, bn, 2, stream);
-            else rc = (precision == 1) ? launch_tc<128, 4, 0, true, 1>(ma, mb, p, grid, stream)
-                                       : launch_tc<128, 5, 0, true, 0>(ma, mb, p, grid, stream);
+            CUtensorMap mo, mr;   // TMA epilogue: the parity class of dx (and residual / mask) as (Cin, Wc, Hc, B, 1)
+            memset(&mo, 0, sizeof(mo));
+            memset(&mr, 0, sizeof(mr));
+            rc = setup_epi_px(p, &mo, &mr, (size_t)(py * W + px) * Cin, Wc, Hc, B, (uint64_t)stride * Cin,
+                              (uint64_t)stride * W * Cin, (uint64_t)H * W * Cin, 1);
+            if (rc) return rc;
+            if (bf) rc = launch_fwd(ma, mb, mo, mr, p, grid, bn, 2, stream);
+            else rc = (precision == 1) ? launch_tc<128, 4, 0, true, 1>(ma, mb, mo, mr, p, grid, stream)
+                                       : launch_tc<128, 5, 0, true, 0>(ma, mb, mo, mr, p, grid, stream);
             if (rc) return rc;
         }
     return 0;
@@ -866,10 +1010,15 @@ int mdb_conv2d_wgrad_bias_f32(const float* dy, const float* x, const float* rows
         rc = make_map(&mb, x, 4, dims, str, box, es);
         if (rc) return rc;
     }
+    // The split partial tiles are added by the register epilogue's vector reds: a bulk tensor reduction of the staged
+    // tile (cp.reduce.async.bulk.tensor) measured slower on the H100 at the model's small-M shapes.
+    CUtensorMap mo, mr;
+    memset(&mo, 0, sizeof(mo));
+    memset(&mr, 0, sizeof(mr));
     dim3 grid((Cin + bn - 1) / bn, (Cout + BM - 1) / BM, taps * splits);
-    rc = g_precision == 2 ? launch_tc<128, 4, 1, true, 2>(ma, mb, p, grid, stream)
-         : g_precision == 1 ? launch_tc<128, 4, 1, true, 1>(ma, mb, p, grid, stream)
-                            : launch_tc<128, 5, 1, true, 0>(ma, mb, p, grid, stream);
+    rc = g_precision == 2 ? launch_tc<128, 4, 1, true, 2>(ma, mb, mo, mr, p, grid, stream)
+         : g_precision == 1 ? launch_tc<128, 4, 1, true, 1>(ma, mb, mo, mr, p, grid, stream)
+                            : launch_tc<128, 5, 1, true, 0>(ma, mb, mo, mr, p, grid, stream);
     if (rc) return rc;
     return 0;
 }

@@ -1,7 +1,11 @@
-"""GPU micro-benchmark of the wgmma conv/linear family on the model's real shapes (B=8), both precision modes."""
+"""GPU micro-benchmark of the wgmma conv/linear family on the model's real shapes (B=8), both precision modes.
+
+--tile-probe: the per-tile fixed cost of the GEMM instead (see tile_probe)."""
 import os
+import subprocess
 import sys
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -36,6 +40,78 @@ def timeit(fn, n=10):
     torch.cuda.synchronize()
     return e0.elapsed_time(e1) / n * 1e3   # us
 
+
+def card():
+    q = "name,power.limit,clocks.sm,clocks.max.sm,clocks_throttle_reasons.active"
+    try:
+        return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True,
+                              timeout=30).stdout.strip().splitlines()[0] + f"  ({q})"
+    except (OSError, subprocess.SubprocessError, IndexError):
+        return torch.cuda.get_device_name()
+
+
+def wgrad_schedule(M, Cin, Cout, sms):
+    """(tiles per CTA, k-blocks per tile) of a pointwise wgrad launch: restates the split rule of mdb_conv2d_wgrad_bias_f32."""
+    total_red = (M + 31) // 32
+    tiles = ((Cout + 127) // 128) * ((Cin + 127) // 128)
+    big, small = min((2 * sms + tiles - 1) // tiles, total_red // 24), min(sms // tiles, total_red // 8)
+    per = -(-total_red // max(big, small, 1))
+    n = tiles * -(-total_red // per)
+    return -(-n // min(n, sms)), per
+
+
+def fit(rows):
+    """Least squares t = fixed * tiles_per_cta + per_kb * tiles_per_cta * kb over rows of (tiles_per_cta, kb, t)."""
+    X = np.array([[tpc, tpc * kb] for tpc, kb, _ in rows], dtype=np.float64)
+    (fixed, per_kb), *_ = np.linalg.lstsq(X, np.array([t for *_, t in rows]), rcond=None)
+    return fixed, per_kb
+
+
+def tile_probe():
+    """Per-tile fixed cost of tc_conv_gemm_kernel (BF16x3) at the encoder size M = 81 600, N = 256.  K (the reduction, 1-8
+    k-blocks of 32) varies at a constant tile count, so the fit t = tiles_per_cta * (fixed + kb * per_kb) separates the
+    cost of a tile's k-blocks from what a tile costs whatever its K (epilogue, tile switch; the launch is in it too).
+    wgrad varies M instead, which changes both its split count and the k-blocks per split."""
+    tc.set_precision("bf16x3")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    M, N = 81600, 256
+    tpc = -(-(-(-M // 128) * (N // 128)) // sms)
+    print(f"== tile probe: {card()}; {sms} SMs, M = {M}, N = {N}, {tpc} tiles per CTA in fwd / dgrad")
+    res = {"fwd": [], "fwd+res": [], "dgrad+mask": [], "wgrad": []}
+    for K in (32, 64, 128, 256):
+        x = torch.randn(M, K, device="cuda")
+        w = tc.split_weights([torch.randn(N, K, 1, 1, device="cuda") / K ** 0.5])[0]
+        wd = tc.split_weights([torch.randn(K, N, 1, 1, device="cuda") / N ** 0.5])[0]   # layer N -> K: its dgrad writes N
+        r = torch.randn(M, N, device="cuda")
+        dy = torch.randn(M, K, device="cuda")
+        x4, r4, dy4 = x.view(1, 1, M, K), r.view(1, 1, M, N), dy.view(1, 1, M, K)
+        kb = K // 32
+        t_f = timeit(lambda: tc.conv2d_forward(x4, w), 50)
+        t_fr = timeit(lambda: tc.conv2d_forward(x4, w, None, r4, relu=True), 50)
+        t_d = timeit(lambda: tc.conv2d_dgrad(dy4, wd, (1, 1, M, N), r4, r4), 50)
+        floor = lambda nbytes: nbytes / 3.35e6   # us at the data-sheet 3.35 TB/s
+        out_b, in_b = M * N * 4, M * K * 4
+        res["fwd"].append((tpc, kb, t_f))
+        res["fwd+res"].append((tpc, kb, t_fr))
+        res["dgrad+mask"].append((tpc, kb, t_d))
+        print(f"K = {K:3d}: fwd {t_f:7.1f} us (HBM floor {floor(in_b + out_b):5.1f})  fwd+res+relu {t_fr:7.1f} "
+              f"(floor {floor(in_b + 2 * out_b):5.1f})  dgrad+res+mask {t_d:7.1f} (floor {floor(in_b + 3 * out_b):5.1f})")
+    for Mw in (10200, 20400, 40800, 81600):
+        dy, x = torch.randn(1, 1, Mw, N, device="cuda"), torch.randn(1, 1, Mw, N, device="cuda")
+        t_w = timeit(lambda: tc.conv2d_wgrad(dy, x), 50)
+        wt, wkb = wgrad_schedule(Mw, N, N, sms)
+        res["wgrad"].append((wt, wkb, t_w))
+        print(f"wgrad {N}x{N} over M = {Mw:5d}: {t_w:7.1f} us ({wt} tiles per CTA, {wkb} k-blocks per tile)")
+    for name, rows in res.items():
+        fixed, per_kb = fit(rows)
+        t_enc = rows[-1][2]
+        print(f"{name:11s} fixed {fixed:6.2f} us/tile, {per_kb:6.3f} us/k-block;  at the largest point fixed x tiles per CTA = "
+              f"{fixed * rows[-1][0]:6.1f} us of {t_enc:6.1f} us ({100 * fixed * rows[-1][0] / t_enc:4.1f} %)")
+
+
+if "--tile-probe" in sys.argv:
+    tile_probe()
+    sys.exit(0)
 
 for mode in tuple(os.environ["MDB_MODES"].split(",")) if os.environ.get("MDB_MODES") else (("tf32x3",) if os.environ.get("MDB_ONLY_X3") else ("bf16x3", "tf32x3", "tf32")):
     tc.set_precision(mode)
