@@ -79,13 +79,15 @@ __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__
 
 // Shared memory of one kernel instance: the TMA ring, the epilogue staging tile of fprop / dgrad (two warpgroups x 64 rows
 // x BN fp32, as 32-channel boxes of 64 128-byte swizzled rows) when it fits beside the ring, the consumers' B operand
-// tile(s), barriers.
+// tile(s) -- two sets, by k-block parity, so that one k-block's wgmmas can read one while the next k-block's B is written
+// into the other --, barriers.
 template <int BN, int STAGES, int MODE, int PREC>
 struct TcSmem {
     static constexpr bool kConvB = !(PREC == 2 && MODE == 0);
     static constexpr int kRing = STAGES * (kTileABytes + BN * 128);
     static constexpr int kStage = 2 * 64 * BN * 4;
-    static constexpr int kConv = kConvB ? (PREC == 1 ? 2 : 1) * BN * 128 : 0;
+    static constexpr int kConvBuf = kConvB ? (PREC == 1 ? 2 : 1) * BN * 128 : 0;   // [hi | lo] operand tiles of one k-block
+    static constexpr int kConv = 2 * kConvBuf;
     static constexpr int kFixed = kRing + kConv + 1024 /*align slack*/ + 256 /*barriers*/;
     static constexpr bool kTmaEpi = MODE == 0 && kFixed + kStage <= 227 * 1024;
     static constexpr int kBytes = kFixed + (kTmaEpi ? kStage : 0);
@@ -96,7 +98,10 @@ struct TcSmem {
 //   warps 0-7       two consumer warpgroups; warpgroup g owns rows [64g, 64g+64) of the 128-row tile.  Per k-block each
 //                   thread loads its A fragments from the landed fp32 tile and splits them in registers; B is read by the
 //                   tensor core from shared memory, either as delivered (pre-split bf16 weights) or after the consumers
-//                   have rewritten it into a K-major operand tile (see CONVB).
+//                   have rewritten it into a K-major operand tile (see CONVB).  The consumer loop is software-pipelined:
+//                   k-block i's wgmmas run while the thread waits for k-block i+1's stage and loads it into the other of
+//                   two fragment buffers (and B operand tiles); the stage of k-block i-1 is released once its wgmmas are
+//                   known complete.  Every accumulator still sees the same wgmmas in the same k order.
 // PREC (arithmetic):
 //   2  bf16x3: x = hi + lo with hi = bf16(x), lo = bf16(x - hi); per k-block A_hi*B_hi + A_lo*B_hi + A_hi*B_lo as
 //      m64nBNk16 bf16 wgmma.  In fprop / dgrad the B operand arrives PRE-SPLIT from global memory -- packed weights
@@ -122,7 +127,7 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
 
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* stage_out = smem + STAGES * kRawBytes;               // epilogue staging tile (SM::kTmaEpi)
-    uint8_t* bconv = stage_out + (SM::kTmaEpi ? SM::kStage : 0);  // [hi | lo] operand tiles of the current k-block (CONVB)
+    uint8_t* bconv = stage_out + (SM::kTmaEpi ? SM::kStage : 0);  // [hi | lo] operand tiles of even / odd k-blocks (CONVB)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(bconv + SM::kConv);
     uint64_t* empty_bar = full_bar + STAGES;
     uint64_t* epi_bar = empty_bar + STAGES;                       // per warpgroup: its residual / mask box has landed
@@ -251,6 +256,128 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     const bool leader = (ctid & 127) == 0;
     uint8_t* my_stage = stage_out + wg * (SM::kStage / 2);
     uint32_t epi_phase = 0;
+    constexpr int KS = PREC == 2 ? 2 : 4;                         // k-steps per k-block: 16 bf16 or 8 tf32 each
+    using Frag = uint32_t[KS][4];                                 // this thread's A fragments of one k-block (hi or lo)
+    // Wait for ring k-block gi, rewrite its B into operand tile set `buf` (CONVB), then load this thread's A fragments of it
+    // and split them into hi / lo.
+    auto load_kblock = [&](int gi, int buf, Frag& hi, Frag& lo) {
+        const int s = gi % STAGES;
+        mbar_wait(&full_bar[s], (gi / STAGES) & 1);
+        const uint8_t* a_raw = smem + s * kRawBytes;
+        if constexpr (CONVB) {
+            const uint8_t* b_raw = a_raw + kTileABytes;
+            uint8_t* bc = bconv + buf * SM::kConvBuf;
+            // Every consumer has waited for the wgmmas that last read this operand tile set (k-block gi - 2's, or the
+            // previous tile's): it may be rewritten.
+            named_bar_sync(1, kConsumerThreads);
+            if constexpr (PREC == 2) {
+                // B -> K-major bf16 rows [hi 32 | lo 32] (the packed-weight format): item = (n, 8-element k group c)
+#pragma unroll
+                for (int i = ctid; i < BN * 4; i += kConsumerThreads) {
+                    const int n = i % BN, c = i / BN;
+                    float x[8];
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) x[e] = *reinterpret_cast<const float*>(b_raw + raw_off<B_MN>(n, 8 * c + e));
+                    uint32_t hw[4], lw[4];
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const uint32_t h = pack_bf16x2(x[2 * e], x[2 * e + 1]);
+                        hw[e] = h;
+                        lw[e] = pack_bf16x2(x[2 * e] - __uint_as_float(h << 16), x[2 * e + 1] - __uint_as_float(h & 0xFFFF0000u));
+                    }
+                    uint8_t* brow = bc + n * 128;
+                    *reinterpret_cast<uint4*>(brow + ((c ^ (n & 7)) << 4)) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+                    *reinterpret_cast<uint4*>(brow + (((4 + c) ^ (n & 7)) << 4)) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+                }
+            } else {
+                // B -> K-major tf32 hi tile (+ lo tile for 3xTF32): item = (n, 4-element k group c)
+#pragma unroll 4
+                for (int i = ctid; i < BN * 8; i += kConsumerThreads) {
+                    const int n = i % BN, c = i / BN;
+                    float4 x;
+                    if constexpr (B_MN) {
+                        x.x = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c));
+                        x.y = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c + 1));
+                        x.z = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c + 2));
+                        x.w = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c + 3));
+                    } else {
+                        x = *reinterpret_cast<const float4*>(b_raw + raw_off<false>(n, 4 * c));
+                    }
+                    const float4 h = make_float4(trunc_tf32(x.x), trunc_tf32(x.y), trunc_tf32(x.z), trunc_tf32(x.w));
+                    const uint32_t off = n * 128 + ((c ^ (n & 7)) << 4);
+                    *reinterpret_cast<float4*>(bc + off) = h;
+                    if constexpr (PREC == 1)
+                        *reinterpret_cast<float4*>(bc + kTileBBytes + off) = make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
+                }
+            }
+            fence_proxy_async_smem();      // generic-proxy writes -> visible to the tensor core's async-proxy reads
+            named_bar_sync(1, kConsumerThreads);
+        }
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+            for (int f = 0; f < 4; ++f) {
+                const int row = r0 + (f & 1) * 8;
+                if constexpr (PREC == 2) {
+                    // fragment f: rows + 8 * (f & 1), k pair 2 * tig + 8 * (f >> 1) of this 16-wide step
+                    const int k = ks * 16 + tig * 2 + (f >> 1) * 8;
+                    float x0, x1;
+                    if constexpr (A_MN) {
+                        x0 = *reinterpret_cast<const float*>(a_raw + raw_off<true>(row, k));
+                        x1 = *reinterpret_cast<const float*>(a_raw + raw_off<true>(row, k + 1));
+                    } else {
+                        const float2 v = *reinterpret_cast<const float2*>(a_raw + raw_off<false>(row, k));
+                        x0 = v.x; x1 = v.y;
+                    }
+                    const uint32_t h = pack_bf16x2(x0, x1);
+                    hi[ks][f] = h;
+                    lo[ks][f] = pack_bf16x2(x0 - __uint_as_float(h << 16), x1 - __uint_as_float(h & 0xFFFF0000u));
+                } else {
+                    // fragment f: rows + 8 * (f & 1), k = tig + 4 * (f >> 1) of this 8-wide step
+                    const int k = ks * 8 + tig + (f >> 1) * 4;
+                    const float x = *reinterpret_cast<const float*>(a_raw + raw_off<A_MN>(row, k));
+                    const float h = trunc_tf32(x);
+                    hi[ks][f] = __float_as_uint(h);
+                    lo[ks][f] = __float_as_uint(x - h);
+                }
+            }
+        }
+    };
+    // Issue ring k-block gi's wgmmas (B from its stage, or from operand tile set `buf`) as one commit group.
+    auto issue_kblock = [&](int gi, int buf, const Frag& hi, const Frag& lo, float (&acc)[NACC]) {
+        const uint32_t b_addr = smem_u32(CONVB ? bconv + buf * SM::kConvBuf : smem + (gi % STAGES) * kRawBytes + kTileABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            // B hi at byte 32 * ks of each 128-byte row; bf16 lo at 64 + 32 * ks, tf32 lo in the second tile
+            const uint64_t bhi = make_wgmma_desc_sw128(b_addr + ks * 32);
+            const uint64_t blo = make_wgmma_desc_sw128(b_addr + (PREC == 2 ? 64 : kTileBBytes) + ks * 32);
+            if constexpr (PREC == 2) {
+                if constexpr (BN == 128) {
+                    wgmma_bf16_n128(acc, hi[ks], bhi, 1);
+                    wgmma_bf16_n128(acc, lo[ks], bhi, 1);
+                    wgmma_bf16_n128(acc, hi[ks], blo, 1);
+                } else {
+                    wgmma_bf16_n64(acc, hi[ks], bhi, 1);
+                    wgmma_bf16_n64(acc, lo[ks], bhi, 1);
+                    wgmma_bf16_n64(acc, hi[ks], blo, 1);
+                }
+            } else {
+                if constexpr (BN == 128) wgmma_tf32_n128(acc, hi[ks], bhi, 1);
+                else wgmma_tf32_n64(acc, hi[ks], bhi, 1);
+                if constexpr (PREC == 1) {
+                    if constexpr (BN == 128) {
+                        wgmma_tf32_n128(acc, lo[ks], bhi, 1);
+                        wgmma_tf32_n128(acc, hi[ks], blo, 1);
+                    } else {
+                        wgmma_tf32_n64(acc, lo[ks], bhi, 1);
+                        wgmma_tf32_n64(acc, hi[ks], blo, 1);
+                    }
+                }
+            }
+        }
+        wgmma_commit();
+    };
     int git = 0;
     for (int tix = blockIdx.x; tix < p.total_tiles; tix += gridDim.x) {
         const Tile t = decode(tix);
@@ -268,133 +395,54 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
         float acc[NACC];
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
-        for (int it = 0; it < t.iters; ++it, ++git) {
-            const int s = git % STAGES;
-            const uint32_t ph = (git / STAGES) & 1;
-            mbar_wait(&full_bar[s], ph);
-            const uint8_t* a_raw = smem + s * kRawBytes;
-            const uint8_t* b_raw = a_raw + kTileABytes;
-            if constexpr (CONVB) {
-                // Every consumer has waited for its MMAs of the previous k-block: the operand tile(s) may be rewritten.
-                named_bar_sync(1, kConsumerThreads);
-                if constexpr (PREC == 2) {
-                    // B -> K-major bf16 rows [hi 32 | lo 32] (the packed-weight format): item = (n, 8-element k group c)
-#pragma unroll
-                    for (int i = ctid; i < BN * 4; i += kConsumerThreads) {
-                        const int n = i % BN, c = i / BN;
-                        float x[8];
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) x[e] = *reinterpret_cast<const float*>(b_raw + raw_off<B_MN>(n, 8 * c + e));
-                        uint32_t hw[4], lw[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const uint32_t h = pack_bf16x2(x[2 * e], x[2 * e + 1]);
-                            hw[e] = h;
-                            lw[e] = pack_bf16x2(x[2 * e] - __uint_as_float(h << 16), x[2 * e + 1] - __uint_as_float(h & 0xFFFF0000u));
-                        }
-                        uint8_t* brow = bconv + n * 128;
-                        *reinterpret_cast<uint4*>(brow + ((c ^ (n & 7)) << 4)) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-                        *reinterpret_cast<uint4*>(brow + (((4 + c) ^ (n & 7)) << 4)) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-                    }
-                } else {
-                    // B -> K-major tf32 hi tile (+ lo tile for 3xTF32): item = (n, 4-element k group c)
-#pragma unroll 4
-                    for (int i = ctid; i < BN * 8; i += kConsumerThreads) {
-                        const int n = i % BN, c = i / BN;
-                        float4 x;
-                        if constexpr (B_MN) {
-                            x.x = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c));
-                            x.y = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c + 1));
-                            x.z = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c + 2));
-                            x.w = *reinterpret_cast<const float*>(b_raw + raw_off<true>(n, 4 * c + 3));
-                        } else {
-                            x = *reinterpret_cast<const float4*>(b_raw + raw_off<false>(n, 4 * c));
-                        }
-                        const float4 h = make_float4(trunc_tf32(x.x), trunc_tf32(x.y), trunc_tf32(x.z), trunc_tf32(x.w));
-                        const uint32_t off = n * 128 + ((c ^ (n & 7)) << 4);
-                        *reinterpret_cast<float4*>(bconv + off) = h;
-                        if constexpr (PREC == 1)
-                            *reinterpret_cast<float4*>(bconv + kTileBBytes + off) = make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
-                    }
+        if (t.iters > 0) {
+            // Two fragment buffers (and operand tile sets) by k-block parity: k-block it's wgmmas run while k-block it + 1
+            // is loaded into the other buffer.  A stage is released after the wait that retires its wgmmas.
+            Frag ahi0, alo0, ahi1, alo1;
+            auto step = [&](int it, const Frag& chi, const Frag& clo, Frag& nhi, Frag& nlo) {
+                issue_kblock(git + it, it & 1, chi, clo, acc);
+                wgmma_wait<1>();                                  // k-block it - 1's wgmmas have completed:
+                wgmma_fence_operands(nhi);                        // its fragments may be overwritten
+                wgmma_fence_operands(nlo);
+                if (it > 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[(git + it - 1) % STAGES]);   // this warp is done with the stage
                 }
-                fence_proxy_async_smem();      // generic-proxy writes -> visible to the tensor core's async-proxy reads
-                named_bar_sync(1, kConsumerThreads);
+                if (it + 1 < t.iters) load_kblock(git + it + 1, (it + 1) & 1, nhi, nlo);
+            };
+            load_kblock(git, 0, ahi0, alo0);
+            for (int it = 0; it < t.iters; it += 2) {
+                step(it, ahi0, alo0, ahi1, alo1);
+                if (it + 1 < t.iters) step(it + 1, ahi1, alo1, ahi0, alo0);
             }
-            const uint32_t b_addr = smem_u32(CONVB ? bconv : b_raw);
-            // All A fragments of the k-block are loaded and split before the first wgmma: registers an in-flight wgmma
-            // reads must not be written until it completes.
-            constexpr int KS = PREC == 2 ? 2 : 4;                 // k-steps per k-block: 16 bf16 or 8 tf32 each
-            uint32_t ahi[KS][4], alo[KS][4];
-#pragma unroll
-            for (int ks = 0; ks < KS; ++ks) {
-#pragma unroll
-                for (int f = 0; f < 4; ++f) {
-                    const int row = r0 + (f & 1) * 8;
-                    if constexpr (PREC == 2) {
-                        // fragment f: rows + 8 * (f & 1), k pair 2 * tig + 8 * (f >> 1) of this 16-wide step
-                        const int k = ks * 16 + tig * 2 + (f >> 1) * 8;
-                        float x0, x1;
-                        if constexpr (A_MN) {
-                            x0 = *reinterpret_cast<const float*>(a_raw + raw_off<true>(row, k));
-                            x1 = *reinterpret_cast<const float*>(a_raw + raw_off<true>(row, k + 1));
-                        } else {
-                            const float2 v = *reinterpret_cast<const float2*>(a_raw + raw_off<false>(row, k));
-                            x0 = v.x; x1 = v.y;
-                        }
-                        const uint32_t h = pack_bf16x2(x0, x1);
-                        ahi[ks][f] = h;
-                        alo[ks][f] = pack_bf16x2(x0 - __uint_as_float(h << 16), x1 - __uint_as_float(h & 0xFFFF0000u));
-                    } else {
-                        // fragment f: rows + 8 * (f & 1), k = tig + 4 * (f >> 1) of this 8-wide step
-                        const int k = ks * 8 + tig + (f >> 1) * 4;
-                        const float x = *reinterpret_cast<const float*>(a_raw + raw_off<A_MN>(row, k));
-                        const float h = trunc_tf32(x);
-                        ahi[ks][f] = __float_as_uint(h);
-                        alo[ks][f] = __float_as_uint(x - h);
-                    }
-                }
-            }
-            wgmma_fence();
-#pragma unroll
-            for (int ks = 0; ks < KS; ++ks) {
-                // B hi at byte 32 * ks of each 128-byte row; bf16 lo at 64 + 32 * ks, tf32 lo in the second tile
-                const uint64_t bhi = make_wgmma_desc_sw128(b_addr + ks * 32);
-                const uint64_t blo = make_wgmma_desc_sw128(b_addr + (PREC == 2 ? 64 : kTileBBytes) + ks * 32);
-                if constexpr (PREC == 2) {
-                    if constexpr (BN == 128) {
-                        wgmma_bf16_n128(acc, ahi[ks], bhi, 1);
-                        wgmma_bf16_n128(acc, alo[ks], bhi, 1);
-                        wgmma_bf16_n128(acc, ahi[ks], blo, 1);
-                    } else {
-                        wgmma_bf16_n64(acc, ahi[ks], bhi, 1);
-                        wgmma_bf16_n64(acc, alo[ks], bhi, 1);
-                        wgmma_bf16_n64(acc, ahi[ks], blo, 1);
-                    }
-                } else {
-                    if constexpr (BN == 128) wgmma_tf32_n128(acc, ahi[ks], bhi, 1);
-                    else wgmma_tf32_n64(acc, ahi[ks], bhi, 1);
-                    if constexpr (PREC == 1) {
-                        if constexpr (BN == 128) {
-                            wgmma_tf32_n128(acc, alo[ks], bhi, 1);
-                            wgmma_tf32_n128(acc, ahi[ks], blo, 1);
-                        } else {
-                            wgmma_tf32_n64(acc, alo[ks], bhi, 1);
-                            wgmma_tf32_n64(acc, ahi[ks], blo, 1);
-                        }
-                    }
-                }
-            }
-            wgmma_commit();
-            wgmma_wait_all();
+            wgmma_wait<0>();
             wgmma_fence_operands(acc);
+            wgmma_fence_operands(ahi0);
+            wgmma_fence_operands(alo0);
+            wgmma_fence_operands(ahi1);
+            wgmma_fence_operands(alo1);
             __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[s]);            // this warp is done with the stage
+            if (lane == 0) mbar_arrive(&empty_bar[(git + t.iters - 1) % STAGES]);
+            git += t.iters;
         }
 
         if (epi_tma) {
             // ---- TMA epilogue: the same operations in the same order as the register epilogue below, through the
             // staging tile (which holds the TMA-fetched residual or mask, read in place); the map clips the box at the
             // output's bounds, so rows and channels past them are computed but never stored.
+            // Operands read from global memory (the bias; a mask beside a TMA-fetched residual) are loaded in batches with no
+            // staging-tile store in between: a load placed after such a store is not moved above it (the compiler cannot
+            // tell the two apart), which made every 8 columns one more global round trip.  The bias goes into the
+            // accumulators first -- the same addition, in the same order, as below.
+            if (p.bias) {
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int n = t.n0 + j * 8 + tig * 2;         // No % 4 == 0: n < No implies n + 1 < No
+                    if (n >= p.No) continue;
+                    const float b0 = p.bias[n], b1 = p.bias[n + 1];
+                    acc[4 * j] += b0; acc[4 * j + 1] += b1; acc[4 * j + 2] += b0; acc[4 * j + 3] += b1;
+                }
+            }
             if (p.epi_load) {
                 mbar_wait(&epi_bar[wg], epi_phase);
                 epi_phase ^= 1;
@@ -402,6 +450,7 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
                 if (leader) bulk_wait_read_all();
                 named_bar_sync(2 + wg, 128);
             }
+            constexpr int kMB = 8;                                // mask columns groups per batch (registers: 2 x kMB)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = r0 + h * 8, rr = row - 64 * wg;
@@ -414,22 +463,28 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
                         gmask = p.relu_mask + (size_t)((img * p.out_H + y * p.out_sy + p.out_oy) * p.out_W + x * p.out_sx + p.out_ox) * p.ldo;
                 }
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j) {
-                    const int n = t.n0 + j * 8 + tig * 2;         // No % 4 == 0: n < No implies n + 1 < No
-                    if (n >= p.No) continue;
-                    float2* sp = reinterpret_cast<float2*>(my_stage + (j >> 2) * 8192 + raw_off<false>(rr, (j & 3) * 8 + tig * 2));
-                    float v[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};   // (the register path's * 1.f: exact)
-                    if (p.bias) { v[0] += p.bias[n]; v[1] += p.bias[n + 1]; }
-                    if (p.epi_load == 1) { const float2 e = *sp; v[0] += e.x; v[1] += e.y; }
-                    if (p.relu) { v[0] = fmaxf(v[0], 0.f); v[1] = fmaxf(v[1], 0.f); }
-                    if (p.relu_mask) {
-                        float2 m = make_float2(0.f, 0.f);
-                        if (p.epi_load == 2) m = *sp;
-                        else if (gmask) m = *reinterpret_cast<const float2*>(gmask + n);
-                        v[0] = m.x > 0.f ? v[0] : 0.f; v[1] = m.y > 0.f ? v[1] : 0.f;
+                for (int j0 = 0; j0 < BN / 8; j0 += kMB) {
+                    float2 mv[kMB];                               // 0 for rows past the output (computed, never stored)
+#pragma unroll
+                    for (int u = 0; u < kMB; ++u) {
+                        const int n = t.n0 + (j0 + u) * 8 + tig * 2;
+                        mv[u] = (gmask && n < p.No) ? *reinterpret_cast<const float2*>(gmask + n) : make_float2(0.f, 0.f);
                     }
-                    if (p.round_out) { v[0] = round_tf32(v[0]); v[1] = round_tf32(v[1]); }
-                    *sp = make_float2(v[0], v[1]);
+#pragma unroll
+                    for (int u = 0; u < kMB; ++u) {
+                        const int j = j0 + u, n = t.n0 + j * 8 + tig * 2;
+                        if (n >= p.No) continue;
+                        float2* sp = reinterpret_cast<float2*>(my_stage + (j >> 2) * 8192 + raw_off<false>(rr, (j & 3) * 8 + tig * 2));
+                        float v[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};   // (+ bias; the register path's * 1.f: exact)
+                        if (p.epi_load == 1) { const float2 e = *sp; v[0] += e.x; v[1] += e.y; }
+                        if (p.relu) { v[0] = fmaxf(v[0], 0.f); v[1] = fmaxf(v[1], 0.f); }
+                        if (p.relu_mask) {
+                            const float2 m = p.epi_load == 2 ? *sp : mv[u];
+                            v[0] = m.x > 0.f ? v[0] : 0.f; v[1] = m.y > 0.f ? v[1] : 0.f;
+                        }
+                        if (p.round_out) { v[0] = round_tf32(v[0]); v[1] = round_tf32(v[1]); }
+                        *sp = make_float2(v[0], v[1]);
+                    }
                 }
             }
             fence_proxy_async_smem();      // generic-proxy writes -> visible to the bulk copy's async-proxy reads
@@ -660,7 +715,7 @@ int setup_epi_px(TcParams& p, CUtensorMap* mo, CUtensorMap* mr, size_t off, int 
 // Launch the fprop / dgrad kernel (K-major B operand) for the arithmetic mode.
 int launch_fwd(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr, const TcParams& p, dim3 grid, int bn, int precision, cudaStream_t stream) {
     if (precision == 2) return bn == 64 ? launch_tc<64, 6, 0, false, 2>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 2>(ma, mb, mo, mr, p, grid, stream);
-    if (precision == 1) return bn == 64 ? launch_tc<64, 5, 0, false, 1>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 4, 0, false, 1>(ma, mb, mo, mr, p, grid, stream);
+    if (precision == 1) return bn == 64 ? launch_tc<64, 5, 0, false, 1>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 3, 0, false, 1>(ma, mb, mo, mr, p, grid, stream);
     return bn == 64 ? launch_tc<64, 6, 0, false, 0>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 0>(ma, mb, mo, mr, p, grid, stream);
 }
 
@@ -893,7 +948,7 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
                               (uint64_t)stride * W * Cin, (uint64_t)H * W * Cin, 1);
             if (rc) return rc;
             if (bf) rc = launch_fwd(ma, mb, mo, mr, p, grid, bn, 2, stream);
-            else rc = (precision == 1) ? launch_tc<128, 4, 0, true, 1>(ma, mb, mo, mr, p, grid, stream)
+            else rc = (precision == 1) ? launch_tc<128, 3, 0, true, 1>(ma, mb, mo, mr, p, grid, stream)
                                        : launch_tc<128, 5, 0, true, 0>(ma, mb, mo, mr, p, grid, stream);
             if (rc) return rc;
         }

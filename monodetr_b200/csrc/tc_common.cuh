@@ -127,10 +127,22 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Wait until at most N committed wgmma groups of this warp are still pending.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_fence_operands(float (&d)[N]) {   // pins the accumulators across the async MMA
 #pragma unroll
     for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Pins register A fragments: placed after the wait that retires the last wgmma reading them, it keeps the compiler from
+// reusing their registers while that wgmma may still be in flight.
+template <int M, int N>
+__device__ __forceinline__ void wgmma_fence_operands(uint32_t (&a)[M][N]) {
+#pragma unroll
+    for (int i = 0; i < M; ++i)
+#pragma unroll
+        for (int j = 0; j < N; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
 }
 __device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int scale_d) {
     asm volatile(

@@ -50,6 +50,45 @@ def card():
         return torch.cuda.get_device_name()
 
 
+def sm_mhz():
+    """Current SM clock of device 0 in MHz (nvidia-smi), or None."""
+    try:
+        return float(subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                                    capture_output=True, text=True, timeout=30).stdout.split()[0])
+    except (OSError, subprocess.SubprocessError, IndexError, ValueError):
+        return None
+
+
+def pick_tile3(W, H, Bn, n_pix=128):
+    """(tw, th, tb) of an fprop / dgrad M tile: restates pick_tile3 of conv_gemm.cu."""
+    best, res = -1, (n_pix, 1, 1)
+    b = 1
+    while b <= n_pix:
+        w = n_pix // b
+        while w >= 1:
+            h = n_pix // b // w
+            if not (b > 1 and b >= 2 * Bn):
+                cov = -(-W // w) * w * -(-H // h) * h * -(-Bn // b) * b
+                if best < 0 or cov < best:
+                    best, res = cov, (w, h, b)
+            w >>= 1
+        b <<= 1
+    return res
+
+
+def fwd_schedule(H, W, Cin, Cout, k, sms):
+    """(tiles per CTA, k-blocks per tile) of a stride-1 fprop launch (B = 8) with Cin in, Cout out; a dgrad of the layer
+    Cin -> Cout is the fprop Cout -> Cin.  Restates the tile walk of conv_forward_impl (no split-K at these shapes)."""
+    if k == 1:
+        W, H, Bn = B * H * W, 1, 1
+    else:
+        Bn = B
+    tw, th, tb = pick_tile3(W, H, Bn)
+    m_tiles = -(-W // tw) * -(-H // th) * -(-Bn // tb)
+    tiles = m_tiles * -(-Cout // (64 if Cout <= 64 else 128))
+    return -(-tiles // min(tiles, sms)), k * k * -(-Cin // 32)
+
+
 def wgrad_schedule(M, Cin, Cout, sms):
     """(tiles per CTA, k-blocks per tile) of a pointwise wgrad launch: restates the split rule of mdb_conv2d_wgrad_bias_f32."""
     total_red = (M + 31) // 32
@@ -102,10 +141,13 @@ def tile_probe():
         wt, wkb = wgrad_schedule(Mw, N, N, sms)
         res["wgrad"].append((wt, wkb, t_w))
         print(f"wgrad {N}x{N} over M = {Mw:5d}: {t_w:7.1f} us ({wt} tiles per CTA, {wkb} k-blocks per tile)")
+    mhz = sm_mhz()
+    print(f"SM clock sampled after the timings: {mhz} MHz")
     for name, rows in res.items():
         fixed, per_kb = fit(rows)
         t_enc = rows[-1][2]
-        print(f"{name:11s} fixed {fixed:6.2f} us/tile, {per_kb:6.3f} us/k-block;  at the largest point fixed x tiles per CTA = "
+        clk = f" ({per_kb * mhz:5.0f} clk)" if mhz else ""
+        print(f"{name:11s} fixed {fixed:6.2f} us/tile, {per_kb:6.3f} us/k-block{clk};  at the largest point fixed x tiles per CTA = "
               f"{fixed * rows[-1][0]:6.1f} us of {t_enc:6.1f} us ({100 * fixed * rows[-1][0] / t_enc:4.1f} %)")
 
 
@@ -113,9 +155,12 @@ if "--tile-probe" in sys.argv:
     tile_probe()
     sys.exit(0)
 
+sms = torch.cuda.get_device_properties(0).multi_processor_count
+print(f"== {card()}; {sms} SMs.  clk/kb = SM clocks per k-block of 32 (time x SM clock / (tiles per CTA x k-blocks per tile))")
 for mode in tuple(os.environ["MDB_MODES"].split(",")) if os.environ.get("MDB_MODES") else (("tf32x3",) if os.environ.get("MDB_ONLY_X3") else ("bf16x3", "tf32x3", "tf32")):
     tc.set_precision(mode)
     print(f"== {mode}")
+    mhz = None
     for name, H, W, Cin, Cout, k, s in SHAPES:
         x = torch.randn(B, H, W, Cin, device="cuda")
         w = torch.randn(Cout, Cin, k, k, device="cuda") / (Cin * k * k) ** 0.5
@@ -130,5 +175,10 @@ for mode in tuple(os.environ["MDB_MODES"].split(",")) if os.environ.get("MDB_MOD
         t_fr = timeit(lambda: tc.conv2d_forward(x, wp, None, res, k, k, s, pad, relu=True))
         t_d = timeit(lambda: tc.conv2d_dgrad(dy, wp, x.shape, None, x, k, k, s, pad))
         t_w = timeit(lambda: tc.conv2d_wgrad(dy, x, None, k, k, s, pad))
-        print(f"{name:34s} fwd {t_f:7.1f} us ({flop / t_f / 1e6:6.1f} TF/s, {byt / t_f / 1e3:6.0f} GB/s)  fwd+res {t_fr:7.1f}  "
-              f"dgrad+mask {t_d:7.1f} ({flop / t_d / 1e6:6.1f} TF/s)  wgrad {t_w:7.1f} ({flop / t_w / 1e6:6.1f} TF/s)")
+        mhz = mhz or sm_mhz()   # sampled once per mode, right after the first shape's timings
+        clk = lambda t, sched: f"{t * mhz / (sched[0] * sched[1]):5.0f}" if mhz else "  n/a"
+        print(f"{name:34s} fwd {t_f:7.1f} us ({flop / t_f / 1e6:6.1f} TF/s, {byt / t_f / 1e3:6.0f} GB/s, "
+              f"{clk(t_f, fwd_schedule(H, W, Cin, Cout, k, sms))} clk/kb)  fwd+res {t_fr:7.1f}  "
+              f"dgrad+mask {t_d:7.1f} ({flop / t_d / 1e6:6.1f} TF/s, {clk(t_d, fwd_schedule(H, W, Cout, Cin, k, sms))} clk/kb)  "
+              f"wgrad {t_w:7.1f} ({flop / t_w / 1e6:6.1f} TF/s)")
+    print(f"   SM clock sampled: {mhz} MHz")
