@@ -392,6 +392,59 @@ int mdb_photometric_distort_u8(const unsigned char* const* src, const int* src_w
                                const mdb_photometric_params* params, unsigned char* const* dst, const long long* dst_pitch, int B,
                                void* stream);
 
+/* ---- KITTI training targets on the device (labels.cu) ----
+ * The label half of the dataset's __getitem__ (lib/datasets/kitti/kitti_dataset.py:173-330): every label line of a split is parsed
+ * once on the host into a LABEL BANK kept on the device, in CSR form: obj_off (n_bank+1) int64 prefix sums of the per-image line
+ * counts, objects (obj_off[n_bank], MDB_LABEL_RECORD_WIDTH) fp64 records, P2 (n_bank, 3, 4) fp32.  Every line is kept, in file
+ * order (DontCare and unknown classes included): target slot i is line i, as in the reference.  Record columns: */
+#define MDB_LABEL_RECORD_WIDTH 16
+#define MDB_LABEL_CLS 0      /* class code: 0 Pedestrian, 1 Car, 2 Cyclist, -1 any other type */
+#define MDB_LABEL_TRUNC 1    /* truncation, occlusion, alpha: fp64 as parsed */
+#define MDB_LABEL_OCC 2
+#define MDB_LABEL_ALPHA 3
+#define MDB_LABEL_BOX2D 4    /* x1 y1 x2 y2: float32 values (the reference parses box2d as float32) */
+#define MDB_LABEL_HWL 8      /* h w l: fp64 */
+#define MDB_LABEL_POS 11     /* x y z: float32 values */
+#define MDB_LABEL_RY 14      /* fp64; column 15 is unused */
+#define MDB_LABEL_MAX_OBJS 1024
+/* One record per image of the batch, 72 bytes, 8-byte aligned: the draws of kitti_dataset.py:130-154. */
+typedef struct mdb_label_image {
+    double trans[6];    /* 2x3 affine map source image -> network input (get_affine_transform(..., inv=1)[0]), row-major */
+    double crop_scale;  /* 1 when no crop was drawn */
+    int bank_index;     /* image in the bank, 0..n_bank-1 */
+    int img_w, img_h;   /* source image size (the flip mirrors about img_w) */
+    int flip;           /* 0 / 1 */
+} mdb_label_image;
+/* Dataset options (HOST struct, read at launch). */
+#define MDB_DEPTH_NORMAL 0   /* depth = z * crop_scale */
+#define MDB_DEPTH_INVERSE 1  /* depth = z / crop_scale */
+#define MDB_DEPTH_NONE 2     /* depth = z */
+typedef struct mdb_label_config {
+    double mean_size[9];  /* (3 classes, h w l) subtracted from the size; zeros unless `meanshape` */
+    int class_mask;       /* bit c set: class code c is in the writelist */
+    int clip_2d;          /* clip negative l / r / t / b to [0, 1] instead of dropping the object */
+    int depth_scale;      /* MDB_DEPTH_* */
+    int res_w, res_h;     /* network input `resolution` (W, H) */
+    int max_objs;         /* target slots per image, 1..MDB_LABEL_MAX_OBJS (the reference: 50) */
+} mdb_label_config;
+/* Padded targets of B images, one thread per (image, slot), every slot written (zeros where the reference leaves zeros), in the
+ * reference's collated dtypes: calibs (B,S,3,4) f32, indices (B,S) int64 (zeros), labels (B,S) int8, boxes (B,S,4), boxes_3d
+ * (B,S,6), depth (B,S,1), size_2d (B,S,2), size_3d (B,S,3), src_size_3d (B,S,3) f32, heading_bin (B,S,1) int64, heading_res (B,S,1)
+ * f32, mask_2d (B,S) bytes 0 / 1; S = max_objs.  Filters and encoding follow the reference step by step: writelist; level
+ * 'UnKnown' (from the float32 box); z < 2 or > 65; flip of box2d and ry; affine map of the box corners and of the projected 3-d
+ * centre (which must land inside the resolution); l / r / t / b sign test or clip; depth scaling; ry2alpha + angle2class on the
+ * flipped ORIGINAL box; size encoding; mask rule.  Each step runs at the precision numpy 2 gives it there (fp64 with explicit _rn
+ * operations, or float32 _rn), rounded to float32 where the reference stores it; arctan2 is atan2 in fp64 rounded to float32
+ * (numpy's float32 arctan2 is not correctly rounded, so heading_res can differ from the reference's by a few float32 ulp).
+ * obj_off / objects / P2 / images and the outputs are DEVICE arrays; cfg is a HOST pointer.  One launch; the library allocates
+ * nothing.  MDB_EINVAL for a null pointer, B outside 1..65535, n_bank < 1, max_objs outside 1..MDB_LABEL_MAX_OBJS, a non-positive
+ * resolution or an unknown depth_scale.  The image records are read on the device: an image whose bank_index is outside
+ * 0..n_bank-1 gets all-zero targets (monodetr_b200.labels raises ValueError before launching). */
+int mdb_kitti_encode_targets(const long long* obj_off, const double* objects, const float* P2, int n_bank,
+                             const mdb_label_image* images, int B, const mdb_label_config* cfg, float* calibs, long long* indices,
+                             signed char* labels, float* boxes, float* boxes_3d, float* depth, float* size_2d, float* size_3d,
+                             float* src_size_3d, long long* heading_bin, float* heading_res, unsigned char* mask_2d, void* stream);
+
 /* ---- KITTI evaluation on the device (kitti_eval.cu) ----
  * lib/datasets/kitti/kitti_eval_python/eval.py:9-412,614-644 (get_thresholds, clean_data, image_box_overlap, d3_box_overlap,
  * compute_statistics_jit, fused_compute_statistics) and rotate_iou.py:17-330 (the rotated-box IoU).  The annotations of n_img images

@@ -77,6 +77,7 @@ SIGNATURES = {
     "mdb_criterion_losses_backward_f32": [c_int] + [_PTR] * 16 + [c_int] * 5 + [c_float] * 2 + [_PTR] * 8,
     "mdb_warp_affine_normalize_u8": [_PTR] * 5 + [c_int] * 3 + [_PTR] * 4,
     "mdb_photometric_distort_u8": [_PTR] * 6 + [c_int, _PTR],
+    "mdb_kitti_encode_targets": [_PTR] * 3 + [c_int, _PTR, c_int] + [_PTR] * 14,
     "mdb_extract_dets_f32": [_PTR] * 5 + [c_int] * 4 + [_PTR, _PTR],
     "mdb_decode_dets_f32": [_PTR] * 4 + [c_int] * 3 + [c_float, _PTR, _PTR, _PTR],
     "mdb_kitti_overlaps": [_PTR] * 3 + [c_int] * 3 + [ctypes.c_longlong] + [_PTR] * 4,
