@@ -482,6 +482,26 @@ int mdb_kitti_eval(const int* gt_off, const int* dt_off, const long long* ov_off
                    const double* overlaps, const int* classes, const double* min_overlaps, int n_cls, int compute_aos,
                    void* workspace, long long workspace_bytes, double* result, void* stream);
 
+/* Detections of a validation pass kept on the device instead of result files (tester_helper.py:112-132 writes them,
+ * kitti_common.py:294-347 reads them back).  mdb_kitti_collect_dets_f32 takes mdb_decode_dets_f32's rows (B, topk, 14) and
+ * count (B) and writes the count[b] leading rows of image b to position slot[b] of the split:
+ *   table_f (n_img, topk, MDB_KITTI_DT_COLS) fp64 in dt_f's column order, each value rint((double)x * 100) / 100 -- exactly
+ *           float('{:.2f}'.format(x)) of the float32 x, sign of zero included;
+ *   table_cls (n_img, topk) int32: cls_code[int(row class)] (the tester's class name as an eval class code), -1 outside 0..n_code-1;
+ *   slot_info (3, n_img) int32: [0] the count, [1] += 1 per write of the slot (the caller zeroes it per pass and rejects values
+ *           other than 1), [2] 1 when the slot has detections and the first one's printed alpha is not -10 (eval.py:745-751).
+ * slot (B) and cls_code (n_code) are HOST arrays, passed to the kernel by value; a slot outside 0..n_img-1 -> MDB_EINVAL before
+ * any launch.  topk <= MDB_KITTI_MAX_BOXES, n_code <= MDB_KITTI_COLLECT_MAX_CLASSES (else MDB_EUNSUPPORTED).  One launch per
+ * MDB_KITTI_COLLECT_MAX_BATCH images; no synchronisation, no allocation. */
+#define MDB_KITTI_COLLECT_MAX_BATCH 512
+#define MDB_KITTI_COLLECT_MAX_CLASSES 8
+int mdb_kitti_collect_dets_f32(const float* rows, const int* count, const int* slot, int B, int topk, int n_img,
+                               const int* cls_code, int n_code, double* table_f, int* table_cls, int* slot_info, void* stream);
+/* The padded table -> CSR dt_f (n_dt, 13) / dt_cls (n_dt) of mdb_kitti_eval; dt_off (n_img + 1) device int32 prefix sums of the
+ * per-slot counts (slot_info[0]).  One launch. */
+int mdb_kitti_compact_dets(const int* dt_off, const double* table_f, const int* table_cls, int n_img, int topk, double* dt_f,
+                           int* dt_cls, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

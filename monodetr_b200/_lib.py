@@ -84,6 +84,8 @@ SIGNATURES = {
     "mdb_kitti_eval_workspace_bytes": [c_int] * 5,
     "mdb_kitti_eval": [_PTR] * 3 + [c_int] * 5 + [ctypes.c_longlong] + [_PTR] * 7 + [c_int] * 2 + [_PTR, ctypes.c_longlong]
                       + [_PTR, _PTR],
+    "mdb_kitti_collect_dets_f32": [_PTR] * 3 + [c_int] * 3 + [_PTR, c_int] + [_PTR] * 4,
+    "mdb_kitti_compact_dets": [_PTR] * 3 + [c_int] * 2 + [_PTR] * 3,
 }
 _RESTYPES = {"mdb_error_string": ctypes.c_char_p, "mdb_conv2d_forward_workspace_bytes": ctypes.c_longlong,
              "mdb_kitti_eval_workspace_bytes": ctypes.c_longlong}

@@ -502,7 +502,89 @@ int check_sizes(int n_img, int n_gt, int n_dt, int n_cls, int max_gt, int max_dt
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Detections of the validation pass, collected on the device (the path that replaced tester_helper.py:112-132 writing result
+// files and kitti_common.py:294-347 reading them back).  A value goes through the text as '{:.2f}' of the float32 and float()
+// of the text; for a float32 x that is rint(x * 100) / 100 in fp64: the product is exact (24 + 7 significant bits), rint rounds
+// half to even as the formatting does, and the correctly rounded quotient is the double nearest the printed decimal.
+constexpr int kRowCols = 14;                     // mdb_decode_dets_f32: cls, alpha, x0 y0 x1 y1, h w l, X Y Z, ry, score
+constexpr int kCollectBatch = MDB_KITTI_COLLECT_MAX_BATCH;
+__constant__ int kDtFromRow[kDtCols] = {2, 3, 4, 5, 1, 13, 9, 10, 11, 8, 6, 7, 12};   // dt_f column <- row column
+
+__device__ __forceinline__ double text_round(float x) { return __ddiv_rn(rint(__dmul_rn((double)x, 100.0)), 100.0); }
+
+struct CollectArgs {               // by value: the slots were range-checked on the host, no upload is needed
+    int slot[kCollectBatch];
+    int code[MDB_KITTI_COLLECT_MAX_CLASSES];
+    int n_code;
+};
+
+// One CTA per batch image: its count leading rows go to slot slot[b] of the padded table; slot_info (3, n_img) records the count,
+// how many times the slot was written, and whether the first detection's printed alpha differs from -10 (eval.py:745-751).
+__global__ void __launch_bounds__(128) collect_kernel(const float* __restrict__ rows, const int* __restrict__ count, int topk,
+                                                      int n_img, CollectArgs a, double* __restrict__ table_f,
+                                                      int* __restrict__ table_cls, int* __restrict__ slot_info) {
+    const int b = blockIdx.x, s = a.slot[b];
+    const int n = min(max(count[b], 0), topk);
+    const float* r = rows + (size_t)b * topk * kRowCols;
+    double* f = table_f + (size_t)s * topk * kDtCols;
+    for (int i = threadIdx.x; i < n * kDtCols; i += blockDim.x) {
+        const int k = i / kDtCols, c = i - k * kDtCols;
+        f[i] = text_round(r[k * kRowCols + kDtFromRow[c]]);
+    }
+    for (int k = threadIdx.x; k < n; k += blockDim.x) {
+        const int id = (int)r[k * kRowCols];                            // the tester's int(cls_id)
+        table_cls[(size_t)s * topk + k] = id >= 0 && id < a.n_code ? a.code[id] : -1;
+    }
+    if (threadIdx.x == 0) {
+        slot_info[s] = n;
+        atomicAdd(slot_info + n_img + s, 1);
+        slot_info[2 * n_img + s] = n > 0 && text_round(r[1]) != -10.0;
+    }
+}
+
+// The padded table -> the CSR dt_f / dt_cls of mdb_kitti_eval, one CTA per slot.
+__global__ void __launch_bounds__(128) compact_kernel(const int* __restrict__ dt_off, const double* __restrict__ table_f,
+                                                      const int* __restrict__ table_cls, int topk, double* __restrict__ dt_f,
+                                                      int* __restrict__ dt_cls) {
+    const int s = blockIdx.x, d0 = dt_off[s], n = dt_off[s + 1] - d0;
+    const double* f = table_f + (size_t)s * topk * kDtCols;
+    for (int i = threadIdx.x; i < n * kDtCols; i += blockDim.x) dt_f[(size_t)d0 * kDtCols + i] = f[i];
+    for (int k = threadIdx.x; k < n; k += blockDim.x) dt_cls[d0 + k] = table_cls[(size_t)s * topk + k];
+}
+
 }  // namespace
+
+extern "C" int mdb_kitti_collect_dets_f32(const float* rows, const int* count, const int* slot, int B, int topk, int n_img,
+                                          const int* cls_code, int n_code, double* table_f, int* table_cls, int* slot_info,
+                                          void* stream) {
+    if (!rows || !count || !slot || !table_f || !table_cls || !slot_info || (n_code > 0 && !cls_code)) return MDB_EINVAL;
+    if (B < 0 || topk < 1 || n_img < 1 || n_code < 0) return MDB_EINVAL;
+    if (topk > kMaxBoxes || n_code > MDB_KITTI_COLLECT_MAX_CLASSES) return MDB_EUNSUPPORTED;
+    for (int b = 0; b < B; ++b)
+        if (slot[b] < 0 || slot[b] >= n_img) return MDB_EINVAL;
+    CollectArgs a;
+    a.n_code = n_code;
+    for (int c = 0; c < n_code; ++c) a.code[c] = cls_code[c];
+    for (int b0 = 0; b0 < B; b0 += kCollectBatch) {
+        const int nb = min(B - b0, kCollectBatch);
+        for (int b = 0; b < nb; ++b) a.slot[b] = slot[b0 + b];
+        collect_kernel<<<nb, 128, 0, (cudaStream_t)stream>>>(rows + (size_t)b0 * topk * kRowCols, count + b0, topk, n_img, a,
+                                                             table_f, table_cls, slot_info);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return (int)e;
+    }
+    return 0;
+}
+
+extern "C" int mdb_kitti_compact_dets(const int* dt_off, const double* table_f, const int* table_cls, int n_img, int topk,
+                                      double* dt_f, int* dt_cls, void* stream) {
+    if (!dt_off || !table_f || !table_cls || !dt_f || !dt_cls || n_img < 0 || topk < 1) return MDB_EINVAL;
+    if (topk > kMaxBoxes) return MDB_EUNSUPPORTED;
+    if (n_img == 0) return 0;
+    compact_kernel<<<n_img, 128, 0, (cudaStream_t)stream>>>(dt_off, table_f, table_cls, topk, dt_f, dt_cls);
+    return (int)cudaGetLastError();
+}
 
 extern "C" int mdb_kitti_overlaps(const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int max_gt, int max_dt,
                                   long long n_ov, const double* gt_f, const double* dt_f, double* overlaps, void* stream) {

@@ -15,6 +15,10 @@ all images are packed once into CSR tables (`pack`), uploaded in one copy, and e
 back the (tp, fp, fn, similarity) table per score threshold.  Precision, recall, their suffix maxima and the 11- / 40-point AP
 are then computed here in fp64 in the reference's order, so the AP values are bit-identical when the counts are.
 There is no CPU path: without a GPU the call raises.
+
+`GroundTruth` + `DeviceEvaluator` run the validation pass without result files: the decoded detections of each batch are
+collected into a device table (csrc/kitti_eval.cu mdb_kitti_collect_dets_f32), compacted at the end of the pass and evaluated by
+the same kernels (`eval_device_tables`).
 """
 import io
 import logging
@@ -85,34 +89,52 @@ def _col(a, key, n, width=1):
     return np.asarray(a[key], dtype=np.float64).reshape(n, width)
 
 
+def _offsets(counts, dtype=np.int32):
+    return np.concatenate([[0], np.cumsum(counts)]).astype(dtype)
+
+
+def pack_gt(gt_annos):
+    """The ground-truth half of `pack`: gt_off, gt_f, gt_i, n_gt, max_gt and the per-image counts `ng`."""
+    if len(gt_annos) == 0:
+        raise ValueError("kitti_eval: no images")
+    ng = np.array([len(a["name"]) for a in gt_annos], dtype=np.int64)
+    gt_f = [np.concatenate([_col(a, "bbox", n, 4), _col(a, "alpha", n), _col(a, "truncated", n), _col(a, "location", n, 3),
+                            _col(a, "dimensions", n, 3), _col(a, "rotation_y", n)], 1) for a, n in zip(gt_annos, ng)]
+    gt_i = [np.stack([np.asarray(a["occluded"], dtype=np.int64).reshape(n),
+                      np.array([_class_code(s) for s in a["name"]], dtype=np.int64).reshape(n),
+                      np.array([s == "DontCare" for s in a["name"]], dtype=np.int64).reshape(n)], 1) for a, n in zip(gt_annos, ng)]
+    return {"gt_off": _offsets(ng), "ng": ng,
+            "gt_f": np.ascontiguousarray(np.concatenate(gt_f, 0), dtype=np.float64).reshape(-1, GT_COLS),
+            "gt_i": np.ascontiguousarray(np.concatenate(gt_i, 0), dtype=np.int32).reshape(-1, 3),
+            "n_img": len(gt_annos), "n_gt": int(ng.sum()), "max_gt": int(ng.max())}
+
+
+def pack_dt(dt_annos):
+    """The detection half of `pack`: dt_off, dt_f, dt_cls, n_dt, max_dt and the per-image counts `nd`."""
+    nd = np.array([len(a["name"]) for a in dt_annos], dtype=np.int64)
+    dt_f = [np.concatenate([_col(a, "bbox", n, 4), _col(a, "alpha", n), _col(a, "score", n), _col(a, "location", n, 3),
+                            _col(a, "dimensions", n, 3), _col(a, "rotation_y", n)], 1) for a, n in zip(dt_annos, nd)]
+    dt_cls = [np.array([_class_code(s) for s in a["name"]], dtype=np.int64).reshape(n) for a, n in zip(dt_annos, nd)]
+    return {"dt_off": _offsets(nd), "nd": nd,
+            "dt_f": np.ascontiguousarray(np.concatenate(dt_f, 0), dtype=np.float64).reshape(-1, DT_COLS),
+            "dt_cls": np.ascontiguousarray(np.concatenate(dt_cls, 0), dtype=np.int32),
+            "n_dt": int(nd.sum()), "max_dt": int(nd.max())}
+
+
+def pair_sizes(ng, nd):
+    """ov_off (per-image overlap block offsets) and n_ov from the per-image gt / detection counts."""
+    ov_off = _offsets(np.asarray(ng, np.int64) * np.asarray(nd, np.int64), np.int64)
+    return {"ov_off": ov_off, "n_ov": int(ov_off[-1])}
+
+
 def pack(gt_annos, dt_annos):
     """CSR tables of include/monodetr_b200.h (mdb_kitti_*): offsets, gt_f / gt_i / dt_f / dt_cls, and the HOST sizes."""
     if len(gt_annos) != len(dt_annos):
         raise ValueError("kitti_eval: gt_annos and dt_annos must list the same images")
-    if len(gt_annos) == 0:
-        raise ValueError("kitti_eval: no images")
-    ng = np.array([len(a["name"]) for a in gt_annos], dtype=np.int64)
-    nd = np.array([len(a["name"]) for a in dt_annos], dtype=np.int64)
-    gt_off = np.concatenate([[0], np.cumsum(ng)]).astype(np.int32)
-    dt_off = np.concatenate([[0], np.cumsum(nd)]).astype(np.int32)
-    ov_off = np.concatenate([[0], np.cumsum(ng * nd)]).astype(np.int64)
-    gt_f = [np.concatenate([_col(a, "bbox", n, 4), _col(a, "alpha", n), _col(a, "truncated", n), _col(a, "location", n, 3),
-                            _col(a, "dimensions", n, 3), _col(a, "rotation_y", n)], 1) for a, n in zip(gt_annos, ng)]
-    dt_f = [np.concatenate([_col(a, "bbox", n, 4), _col(a, "alpha", n), _col(a, "score", n), _col(a, "location", n, 3),
-                            _col(a, "dimensions", n, 3), _col(a, "rotation_y", n)], 1) for a, n in zip(dt_annos, nd)]
-    gt_i = [np.stack([np.asarray(a["occluded"], dtype=np.int64).reshape(n),
-                      np.array([_class_code(s) for s in a["name"]], dtype=np.int64).reshape(n),
-                      np.array([s == "DontCare" for s in a["name"]], dtype=np.int64).reshape(n)], 1) for a, n in zip(gt_annos, ng)]
-    dt_cls = [np.array([_class_code(s) for s in a["name"]], dtype=np.int64).reshape(n) for a, n in zip(dt_annos, nd)]
-    return {
-        "gt_off": gt_off, "dt_off": dt_off, "ov_off": ov_off,
-        "gt_f": np.ascontiguousarray(np.concatenate(gt_f, 0), dtype=np.float64).reshape(-1, GT_COLS),
-        "gt_i": np.ascontiguousarray(np.concatenate(gt_i, 0), dtype=np.int32).reshape(-1, 3),
-        "dt_f": np.ascontiguousarray(np.concatenate(dt_f, 0), dtype=np.float64).reshape(-1, DT_COLS),
-        "dt_cls": np.ascontiguousarray(np.concatenate(dt_cls, 0), dtype=np.int32),
-        "n_img": len(gt_annos), "n_gt": int(ng.sum()), "n_dt": int(nd.sum()), "n_ov": int(ov_off[-1]),
-        "max_gt": int(ng.max()), "max_dt": int(nd.max()),
-    }
+    g, d = pack_gt(gt_annos), pack_dt(dt_annos)
+    p = {**g, **d, **pair_sizes(g["ng"], d["nd"])}
+    del p["ng"], p["nd"]
+    return p
 
 
 def _device():
@@ -165,20 +187,31 @@ def image_overlaps(gt_annos, dt_annos):
     return out
 
 
-def eval_counts(gt_annos, dt_annos, classes, min_overlaps, compute_aos):
-    """The device pipeline: (n_cfg, 1 + 4 * 41) fp64 table, cfg = ((metric * n_cls + m) * 3 + difficulty) * 2 + k, row =
-    [T, (tp, fp, fn, similarity) per threshold].  Six launches, one upload, one download."""
+def _check_classes(classes, min_overlaps):
     classes = [int(c) for c in classes]
     if not classes or any(c not in CLASS_TO_NAME for c in classes):
         raise ValueError(f"kitti_eval: classes must be codes in 0..5, got {classes}")
     min_overlaps = np.asarray(min_overlaps, dtype=np.float64)
     if min_overlaps.shape != (2, 3, len(classes)):
         raise ValueError("kitti_eval: min_overlaps must have shape (2, 3, len(classes))")
+    return classes, min_overlaps
+
+
+def eval_counts(gt_annos, dt_annos, classes, min_overlaps, compute_aos):
+    """The device pipeline: (n_cfg, 1 + 4 * 41) fp64 table, cfg = ((metric * n_cls + m) * 3 + difficulty) * 2 + k, row =
+    [T, (tp, fp, fn, similarity) per threshold].  Six launches, one upload, one download."""
+    classes, min_overlaps = _check_classes(classes, min_overlaps)
     p = pack(gt_annos, dt_annos)
-    d = _to_device(p, classes, min_overlaps)
+    return eval_device_tables(_to_device(p, classes, min_overlaps), p, len(classes), compute_aos)
+
+
+def eval_device_tables(d, p, n_cls, compute_aos):
+    """The counts table of `eval_counts` from tables already on the device: `d` holds the device arrays gt_off, dt_off, ov_off,
+    gt_f, gt_i, dt_f, dt_cls, classes and min_overlaps, `p` the HOST sizes n_img, n_gt, n_dt, n_ov, max_gt, max_dt.  Every
+    evaluation (annotation lists or the device table of `DeviceEvaluator`) launches the eval kernels here: six launches, one
+    download."""
     dev = d["gt_f"].device
     ov = _launch_overlaps(p, d)
-    n_cls = len(classes)
     need = _lib.lib().mdb_kitti_eval_workspace_bytes(p["n_img"], p["n_gt"], p["n_dt"], n_cls, int(compute_aos))
     if need < 0:
         _lib.check(int(need), "mdb_kitti_eval_workspace_bytes")
@@ -232,8 +265,12 @@ def do_eval(gt_annos, dt_annos, current_classes, min_overlaps, compute_aos=False
     device call."""
     if not DIForDIS:
         raise NotImplementedError("kitti_eval: the distance-binned evaluation (DIForDIS=False) is not implemented")
-    n_cls = len(current_classes)
     table = eval_counts(gt_annos, dt_annos, current_classes, min_overlaps, compute_aos)
+    return _aps(table, len(current_classes), compute_aos, PR_detail_dict)
+
+
+def _aps(table, n_cls, compute_aos, PR_detail_dict=None):
+    """do_eval's result from the counts table."""
     precision, _, aos = _curves(table, n_cls, compute_aos)
     out = {}
     for m, key in enumerate(("bbox", "bev", "3d")):
@@ -254,18 +291,27 @@ def _line(text):
     return s.getvalue()
 
 
-def _official(gt_annos, dt_annos, current_classes, PR_detail_dict=None):
+def _class_codes(current_classes):
     if not isinstance(current_classes, (list, tuple)):
         current_classes = [current_classes]
-    classes = [NAME_TO_CLASS[c] if isinstance(c, str) else c for c in current_classes]
+    return [NAME_TO_CLASS[c] if isinstance(c, str) else c for c in current_classes]
+
+
+def _official(gt_annos, dt_annos, current_classes, PR_detail_dict=None):
+    classes = _class_codes(current_classes)
     min_overlaps = OFFICIAL_MIN_OVERLAPS[:, :, classes]
     compute_aos = False                                     # eval.py:745-751: the first image with detections decides
     for anno in dt_annos:
         if anno["alpha"].shape[0] != 0:
             compute_aos = bool(anno["alpha"][0] != -10)
             break
-    bbox, bev, d3, aos, bbox40, bev40, d340, aos40 = do_eval(gt_annos, dt_annos, classes, min_overlaps, compute_aos,
-                                                             PR_detail_dict=PR_detail_dict)
+    aps = do_eval(gt_annos, dt_annos, classes, min_overlaps, compute_aos, PR_detail_dict=PR_detail_dict)
+    return _report(classes, min_overlaps, aps, compute_aos)
+
+
+def _report(classes, min_overlaps, aps, compute_aos):
+    """get_official_eval_result's per-class result strings, ret_dict and first value from do_eval's arrays."""
+    bbox, bev, d3, aos, bbox40, bev40, d340, aos40 = aps
     texts, ret = [], {}
     for j, c in enumerate(classes):
         name, text = CLASS_TO_NAME[c], ""
@@ -307,7 +353,211 @@ def evaluate(results_dir, label_dir, image_ids, classes=("Car", "Pedestrian", "C
     dt_annos = get_label_annos(results_dir)
     gt_annos = get_label_annos(label_dir, [int(i) for i in image_ids])
     logger.info("==> Evaluating (official) ...")
-    texts, ret, _, codes = _official(gt_annos, dt_annos, list(classes))
+    return _log_result(logger, *_official(gt_annos, dt_annos, list(classes)))
+
+
+def _log_result(logger, texts, ret, first, codes):
     for t in texts:
         logger.info(t)
     return ret["Car_3d_moderate_R40"] if NAME_TO_CLASS["Car"] in codes else 0
+
+
+# ---------------------------------------------------------------------------------------------------------------- validation pass
+TESTER_CLASS_NAMES = ("Pedestrian", "Car", "Cyclist")   # kitti_dataset.py:30: the decode class id indexes this list
+ROW_COLS = 14                                            # decode.OUT_COLS
+COLLECT_MAX_BATCH = 512                                  # MDB_KITTI_COLLECT_MAX_BATCH
+COLLECT_MAX_CLASSES = 8                                  # MDB_KITTI_COLLECT_MAX_CLASSES
+# result-file field order (tester_helper.py:125-132: alpha, bbox, h w l, location, ry, score) as dt_f columns
+_FILE_FROM_DT = [4, 0, 1, 2, 3, 10, 11, 9, 6, 7, 8, 12, 5]
+
+
+_RESULT_LINE = "{} 0.0 0" + " {:.2f}" * DT_COLS + "\n"
+
+
+def result_file_text(rows, class_names):
+    """The text Tester.save_results (tester_helper.py:125-132) writes for one image: rows [class id, value, ...] as
+    decode_detections returns them, the class id indexing `class_names`."""
+    return "".join("{} 0.0 0".format(class_names[int(r[0])]) + "".join(" {:.2f}".format(v) for v in r[1:]) + "\n" for r in rows)
+
+
+def _carve(specs, device):
+    """One device buffer holding several arrays, each 16-byte aligned: (buffer, typed views, byte offsets)."""
+    offs, size = [], 0
+    for dtype, shape in specs:
+        offs.append(size)
+        size += (int(np.prod(shape)) * torch.empty(0, dtype=dtype).element_size() + 15) // 16 * 16
+    buf = torch.zeros(max(size, 16), dtype=torch.uint8, device=device)
+    views = [buf[o:o + int(np.prod(s)) * torch.empty(0, dtype=t).element_size()].view(t).view(*s)
+             for (t, s), o in zip(specs, offs)]
+    return buf, views, offs
+
+
+class GroundTruth:
+    """The labels of a split, parsed once at fp64 (as KITTI_Dataset.eval parses them with kitti_common.get_label_annos) and kept
+    on the device in the CSR form of mdb_kitti_eval, so that every validation pass reuses them.  Image i is the i-th id of
+    `image_ids`."""
+
+    def __init__(self, gt_annos, image_ids=None, device=None):
+        p = pack_gt(gt_annos)
+        self.image_ids = list(range(len(gt_annos))) if image_ids is None else [int(i) for i in image_ids]
+        if len(self.image_ids) != len(gt_annos):
+            raise ValueError("GroundTruth: image_ids and gt_annos must have the same length")
+        self.ng = p["ng"]
+        self.n_img, self.n_gt, self.max_gt = p["n_img"], p["n_gt"], p["max_gt"]
+        self.device = device or _device()
+        self.gt_off, self.gt_f, self.gt_i = _upload([p["gt_off"], p["gt_f"], p["gt_i"]], self.device)
+
+    @classmethod
+    def from_annos(cls, gt_annos, image_ids=None, device=None):
+        return cls(gt_annos, image_ids, device)
+
+    @classmethod
+    def from_kitti(cls, root_dir, split, device=None):
+        """Every image of ImageSets/<split>.txt, labels from training/label_2 (kitti_dataset.py:49-60)."""
+        if split == "test":
+            raise ValueError("GroundTruth.from_kitti: the test split has no labels")
+        with open(os.path.join(root_dir, "ImageSets", split + ".txt")) as f:
+            ids = [int(x.strip()) for x in f.readlines()]
+        return cls(get_label_annos(os.path.join(root_dir, "training", "label_2"), ids), ids, device)
+
+
+class DeviceEvaluator:
+    """One validation pass on the device: the decoded detections of every image go into a padded device table in the form the
+    result files would give them back (values rounded as '{:.2f}' and parsed again), and the KITTI AP is computed from that table
+    with the kernels of `evaluate`.  The result files are only needed for submission (`write_results`).
+
+    Images are paired by their position in the split (`slots`): the reference pairs the sorted ids of its result files with the
+    split's id list, and the two orders agree because KITTI's ImageSets files list ids in ascending order.
+
+      gt           GroundTruth of the split, or None (no `result()`, e.g. the test split: then pass `image_ids`)
+      classes      the classes `result()` evaluates (KITTI_Dataset.writelist), names or codes
+      class_names  the decode class id -> name list of the tester (kitti_dataset.py:30)
+
+    `add` runs extract + decode + collect (three launches on the current stream, no host synchronisation); `result` copies the
+    per-image counts to the host once, compacts the table and runs the eval; `reset` starts the next pass."""
+
+    def __init__(self, gt, classes=("Car",), topk=50, threshold=0.2, cls_mean_size=None, class_names=TESTER_CLASS_NAMES,
+                 image_ids=None, device=None):
+        from .labels import CLS_MEAN_SIZE
+        self.gt = gt
+        if image_ids is None:
+            if gt is None:
+                raise ValueError("DeviceEvaluator: pass a GroundTruth or image_ids")
+            image_ids = gt.image_ids
+        self.image_ids = [int(i) for i in image_ids]
+        if gt is not None and len(self.image_ids) != gt.n_img:
+            raise ValueError("DeviceEvaluator: image_ids must list the images of gt")
+        self.n_img = len(self.image_ids)
+        self.classes = _class_codes(list(classes) if isinstance(classes, (list, tuple)) else classes)
+        self.min_overlaps = OFFICIAL_MIN_OVERLAPS[:, :, self.classes]
+        _check_classes(self.classes, self.min_overlaps)
+        self.class_names = list(class_names)
+        codes = [_class_code(n) for n in self.class_names]
+        if any(c < 0 for c in codes) or len(set(codes)) != len(codes) or len(codes) > COLLECT_MAX_CLASSES:
+            raise ValueError(f"DeviceEvaluator: class_names must be distinct KITTI class names, got {self.class_names}")
+        self.codes = np.array(codes, np.int32)
+        self.topk, self.threshold = int(topk), float(threshold)
+        if not 1 <= self.topk <= MAX_BOXES:
+            raise ValueError(f"DeviceEvaluator: topk must be in 1..{MAX_BOXES}")
+        self.device = device or (gt.device if gt is not None else _device())
+        mean = np.asarray(CLS_MEAN_SIZE if cls_mean_size is None else cls_mean_size, np.float32)
+        self.cls_mean_size = torch.from_numpy(mean).to(self.device)     # uploaded once: a per-batch upload would synchronise
+        self._buf, (self.slot_info, self.table_f, self.table_cls), self._offs = _carve(
+            [(torch.int32, (3, self.n_img)), (torch.float64, (self.n_img, self.topk, DT_COLS)),
+             (torch.int32, (self.n_img, self.topk))], self.device)
+        self._eval_consts = None
+
+    def reset(self):
+        self.slot_info.zero_()
+
+    # ------------------------------------------------------------------------------------------------------------ per batch
+    def add(self, outputs, slots, img_size, calibs):
+        """outputs: MonoDETR.forward's dict of one batch; slots: the batch images' positions in the split (host integers);
+        img_size (B, 2) and calibs (B, 3, 4) or Calibration objects, as decode_detections takes them."""
+        from . import decode
+        dets = decode.extract_dets_from_outputs(outputs, topk=self.topk)
+        rows, count = decode.decode_detections_device(dets, img_size, calibs, self.cls_mean_size, self.threshold)
+        self.add_rows(rows, count, slots)
+
+    def add_rows(self, rows, count, slots):
+        """rows (B, topk, 14) / count (B) as decode_detections_device returns them."""
+        if isinstance(slots, torch.Tensor) and slots.device.type != "cpu":
+            raise TypeError("DeviceEvaluator: slots must be host integers (reading device slots would synchronise)")
+        slots = np.ascontiguousarray(np.asarray(slots, dtype=np.int64).reshape(-1)).astype(np.int32)
+        if rows.shape != (len(slots), self.topk, ROW_COLS) or count.shape != (len(slots),):
+            raise ValueError(f"DeviceEvaluator: rows (B, {self.topk}, {ROW_COLS}) and count (B,) expected for {len(slots)} slots")
+        rows, count = rows.float().contiguous(), count.int().contiguous()
+        with torch.cuda.device(self.device):
+            _lib.call("mdb_kitti_collect_dets_f32", rows, count, slots.ctypes.data, len(slots), self.topk, self.n_img,
+                      self.codes.ctypes.data, len(self.codes), self.table_f, self.table_cls, self.slot_info,
+                      launches=-(-len(slots) // COLLECT_MAX_BATCH))
+
+    # ------------------------------------------------------------------------------------------------------------ end of a pass
+    def _host_info(self, nbytes=None):
+        """One device->host copy of the buffer's first `nbytes` (all of it by default): (slot_info, bytes)."""
+        host = self._buf[:nbytes].cpu().numpy() if nbytes else self._buf.cpu().numpy()
+        info = host[:3 * self.n_img * 4].view(np.int32).reshape(3, self.n_img)
+        added = info[1]
+        if (added != 1).any():
+            twice, missing = np.flatnonzero(added > 1), np.flatnonzero(added == 0)
+            msg = []
+            if len(twice):
+                msg.append(f"{len(twice)} image(s) added more than once (first id {self.image_ids[twice[0]]})")
+            if len(missing):
+                msg.append(f"{len(missing)} image(s) never added (first id {self.image_ids[missing[0]]})")
+            raise ValueError("DeviceEvaluator: " + "; ".join(msg))
+        return info, host
+
+    def counts_table(self):
+        """The (n_cfg, 1 + 4 * 41) counts table of eval_counts for this pass, and compute_aos."""
+        if self.gt is None:
+            raise ValueError("DeviceEvaluator: no GroundTruth, nothing to evaluate against")
+        info, _ = self._host_info(3 * self.n_img * 4)                         # the one synchronisation of the pass
+        nd = info[0].astype(np.int64)
+        with_dets = np.flatnonzero(nd)
+        compute_aos = bool(info[2][with_dets[0]]) if len(with_dets) else False   # eval.py:745-751
+        sizes = {"n_img": self.n_img, "n_gt": self.gt.n_gt, "n_dt": int(nd.sum()), "max_gt": self.gt.max_gt,
+                 "max_dt": int(nd.max()), **pair_sizes(self.gt.ng, nd)}
+        if self._eval_consts is None:
+            self._eval_consts = _upload([np.asarray(self.classes, np.int32), self.min_overlaps], self.device)
+        dt_off, ov_off = _upload([_offsets(nd), sizes["ov_off"]], self.device)
+        dt_f = torch.empty(max(sizes["n_dt"], 1), DT_COLS, dtype=torch.float64, device=self.device)
+        dt_cls = torch.empty(max(sizes["n_dt"], 1), dtype=torch.int32, device=self.device)
+        d = {"gt_off": self.gt.gt_off, "dt_off": dt_off, "ov_off": ov_off, "gt_f": self.gt.gt_f, "gt_i": self.gt.gt_i,
+             "dt_f": dt_f, "dt_cls": dt_cls, "classes": self._eval_consts[0], "min_overlaps": self._eval_consts[1]}
+        with torch.cuda.device(self.device):
+            _lib.call("mdb_kitti_compact_dets", dt_off, self.table_f, self.table_cls, self.n_img, self.topk, dt_f, dt_cls)
+            return eval_device_tables(d, sizes, len(self.classes), compute_aos), compute_aos
+
+    def result(self, logger=None):
+        """What `evaluate` (KITTI_Dataset.eval) returns for this pass -- Car AP3d R40 at moderate difficulty, 0 when 'Car' is not
+        among `classes` -- with the same log lines.  ValueError if an image was added twice or never."""
+        logger = logger or logging.getLogger(__name__)
+        logger.info("==> Loading detections and GTs...")
+        table, compute_aos = self.counts_table()
+        logger.info("==> Evaluating (official) ...")
+        aps = _aps(table, len(self.classes), compute_aos)
+        return _log_result(logger, *_report(self.classes, self.min_overlaps, aps, compute_aos))
+
+    def result_lines(self, class_names=None):
+        """{image id: text of its result file} as the reference's Tester.save_results writes it, from one device->host copy."""
+        names = self.class_names if class_names is None else list(class_names)
+        decode_id = {int(c): i for i, c in enumerate(self.codes)}
+        info, host = self._host_info()
+        f = host[self._offs[1]:self._offs[1] + self.table_f.numel() * 8].view(np.float64).reshape(self.n_img, self.topk, DT_COLS)
+        c = host[self._offs[2]:self._offs[2] + self.table_cls.numel() * 4].view(np.int32).reshape(self.n_img, self.topk)
+        fmt = _RESULT_LINE
+        out = {}
+        for s, img_id in enumerate(self.image_ids):
+            n = int(info[0, s])
+            vals = f[s, :n][:, _FILE_FROM_DT].tolist()
+            out[img_id] = "".join(fmt.format(names[decode_id[int(k)]], *v) for k, v in zip(c[s, :n], vals))
+        return out
+
+    def write_results(self, results_dir, class_names=None):
+        """Writes <results_dir>/%06d.txt for every image, byte-identical to the reference's Tester.save_results
+        (tester_helper.py:112-132) on the same decoded rows.  Works without a GroundTruth (test split)."""
+        os.makedirs(results_dir, exist_ok=True)
+        for img_id, text in self.result_lines(class_names).items():
+            with open(os.path.join(results_dir, "{:06d}.txt".format(img_id)), "w") as f:
+                f.write(text)
