@@ -14,8 +14,8 @@
 // Tile: 128 output pixels (tw x th pixels of tb consecutive images) x BN output channels, K step = 32 fp32
 // (one 128-byte swizzle span).  Persistent CTAs (one per SM) walk the tiles.  Warp roles: warps 0-7 = two consumer
 // warpgroups (64 rows each: operand staging, wgmma, fused epilogue -- through a shared-memory staging tile and TMA
-// stores for fprop / dgrad, straight from the accumulator registers otherwise), warp 8 = TMA producer.  smem ring of
-// STAGES stages, mbarrier full/empty pairs.
+// stores for fprop / dgrad, straight from the accumulator registers otherwise), warpgroup 2 (warps 8-11) = TMA producer,
+// which gives most of its registers to the consumers (setmaxnreg).  smem ring of STAGES stages, mbarrier full/empty pairs.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -36,7 +36,10 @@ constexpr int BK = 32;                 // fp32 elements per k-block = 128 bytes
 constexpr int kTileABytes = BM * 128;  // 16 KiB
 constexpr int kChunkBytes = 32 * 128;  // one MN-major chunk: 32 reduction rows x 128 B
 constexpr int kConsumerThreads = 256;  // two warpgroups
-constexpr int kThreadsTC = kConsumerThreads + 32;
+constexpr int kThreadsTC = kConsumerThreads + 128;   // + the producer warpgroup
+// Registers per thread after reallocation: 128 x 40 + 256 x 232 = 64 512, what 384 threads at 168 start with.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 constexpr int kMaxTaps = 9;
 
 struct TcParams {
@@ -77,24 +80,29 @@ __device__ __forceinline__ uint32_t raw_off(int row, int k) {
 
 __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
-// Shared memory of one kernel instance: the TMA ring, the epilogue staging tile of fprop / dgrad (two warpgroups x 64 rows
-// x BN fp32, as 32-channel boxes of 64 128-byte swizzled rows) when it fits beside the ring, the consumers' B operand
+// Shared memory of one kernel instance: the TMA ring, the epilogue staging tile of fprop / dgrad, the consumers' B operand
 // tile(s) -- two sets, by k-block parity, so that one k-block's wgmmas can read one while the next k-block's B is written
-// into the other --, barriers.
+// into the other --, barriers.  The staging tile is made of 32-channel boxes of 64 128-byte swizzled rows (8 KB), kBufs per
+// warpgroup: all BN / 32 of a warpgroup's 64 x BN results when they fit beside the ring; for BN = 256 (a full staging tile
+// is 128 KB) the largest power of two of them that fits, reused in turn as the stores drain (see the TMA epilogue).
 template <int BN, int STAGES, int MODE, int PREC>
 struct TcSmem {
     static constexpr bool kConvB = !(PREC == 2 && MODE == 0);
     static constexpr int kRing = STAGES * (kTileABytes + BN * 128);
-    static constexpr int kStage = 2 * 64 * BN * 4;
     static constexpr int kConvBuf = kConvB ? (PREC == 1 ? 2 : 1) * BN * 128 : 0;   // [hi | lo] operand tiles of one k-block
     static constexpr int kConv = 2 * kConvBuf;
     static constexpr int kFixed = kRing + kConv + 1024 /*align slack*/ + 256 /*barriers*/;
-    static constexpr bool kTmaEpi = MODE == 0 && kFixed + kStage <= 227 * 1024;
+    static constexpr int kChunks = BN / 32;                        // 32-channel boxes per warpgroup and tile
+    static constexpr int kRoom = (227 * 1024 - kFixed) / (2 * 8192);   // boxes per warpgroup that fit beside the ring
+    static constexpr int kBufs = kRoom >= kChunks ? kChunks : BN < 256 ? 0 : kRoom >= 4 ? 4 : kRoom >= 2 ? 2 : kRoom;
+    static constexpr int kStage = 2 * kBufs * 8192;
+    static constexpr bool kTmaEpi = MODE == 0 && kBufs > 0;
     static constexpr int kBytes = kFixed + (kTmaEpi ? kStage : 0);
 };
 
 // Persistent, warp-specialised kernel.  Each CTA walks tiles  tile = blockIdx.x + i * gridDim.x.
-//   warp 8          TMA producer (smem ring of STAGES stages, full/empty mbarriers)
+//   warps 8-11      producer warpgroup: one thread issues the TMA loads (smem ring of STAGES stages, full/empty mbarriers);
+//                   the warpgroup shrinks to kProducerRegs registers so that the consumers can grow to kConsumerRegs
 //   warps 0-7       two consumer warpgroups; warpgroup g owns rows [64g, 64g+64) of the 128-row tile.  Per k-block each
 //                   thread loads its A fragments from the landed fp32 tile and splits them in registers; B is read by the
 //                   tensor core from shared memory, either as delivered (pre-split bf16 weights) or after the consumers
@@ -104,9 +112,9 @@ struct TcSmem {
 //                   known complete.  Every accumulator still sees the same wgmmas in the same k order.
 // PREC (arithmetic):
 //   2  bf16x3: x = hi + lo with hi = bf16(x), lo = bf16(x - hi); per k-block A_hi*B_hi + A_lo*B_hi + A_hi*B_lo as
-//      m64nBNk16 bf16 wgmma.  In fprop / dgrad the B operand arrives PRE-SPLIT from global memory -- packed weights
-//      [tap][n][k-block][hi 32 | lo 32] bf16, one 128-byte swizzle row per (n, k-block), written once per step by
-//      pack_gemm_weights_bf16x3.  Dropped terms are O(2^-17) per product.
+//      m64nBNk16 bf16 wgmma (BN = 256 only here: 128 accumulators per consumer thread).  In fprop / dgrad the B operand
+//      arrives PRE-SPLIT from global memory -- packed weights [tap][n][k-block][hi 32 | lo 32] bf16, one 128-byte swizzle
+//      row per (n, k-block), written once per step by pack_gemm_weights_bf16x3.  Dropped terms are O(2^-17) per product.
 //   1  3xTF32: hi = trunc_tf32(x), lo = x - hi; the same three products as m64nBNk8 tf32 wgmma.
 //   0  single-pass TF32 (operands truncated by the tensor core; outputs optionally rounded for the next consumer).
 template <int BN, int STAGES, int MODE /*0 fprop/dgrad, 1 wgrad*/, bool B_MN, int PREC>
@@ -116,8 +124,8 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
                     const __grid_constant__ TcParams p) {
     constexpr bool A_MN = (MODE == 1);
     static_assert(!(MODE == 1) || B_MN, "wgrad reads both operands MN-major");
-    static_assert(BN == 64 || BN == 128, "tile width");
     constexpr bool BF_B = (PREC == 2 && MODE == 0);               // B arrives as pre-split bf16 rows
+    static_assert(BN == 64 || BN == 128 || (BN == 256 && BF_B), "tile width");
     static_assert(!BF_B || !B_MN, "pre-split weights are K-major");
     constexpr bool CONVB = !BF_B;                                 // consumers rewrite B into the operand tile(s)
     constexpr int kTileBBytes = BN * 128;
@@ -130,7 +138,12 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     uint8_t* bconv = stage_out + (SM::kTmaEpi ? SM::kStage : 0);  // [hi | lo] operand tiles of even / odd k-blocks (CONVB)
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(bconv + SM::kConv);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* epi_bar = empty_bar + STAGES;                       // per warpgroup: its residual / mask box has landed
+    // TMA epilogue: the warpgroup's staging buffers are used in rounds of kRound boxes, kSlots rounds' worth at a time
+    constexpr int kRound = SM::kBufs >= SM::kChunks ? SM::kChunks : 1;
+    constexpr int kSlots = SM::kBufs / kRound > 0 ? SM::kBufs / kRound : 1;
+    constexpr int kRounds = SM::kChunks / kRound;
+    static_assert(kRounds % kSlots == 0, "every slot serves the same number of rounds per tile");
+    uint64_t* epi_bar = empty_bar + STAGES;                       // [warpgroup][slot]: its residual / mask boxes have landed
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -180,8 +193,7 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], kConsumerThreads / 32);      // one arrival per consumer warp
         }
-        mbar_init(&epi_bar[0], 1);
-        mbar_init(&epi_bar[1], 1);
+        for (int i = 0; i < 2 * kSlots; ++i) mbar_init(&epi_bar[i], 1);
         fence_mbar_init();
     }
     __syncthreads();
@@ -195,9 +207,10 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     // it waits at the same point for this grid to complete.
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-    if (warp == kConsumerThreads / 32) {
+    if (warp >= kConsumerThreads / 32) {
         // ================================ TMA producer =============================================
-        if (elect_one()) {
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp == kConsumerThreads / 32 && elect_one()) {
             int git = 0;                                          // ring position, continues across tiles
             for (int tix = blockIdx.x; tix < p.total_tiles; tix += gridDim.x) {
                 const Tile t = decode(tix);
@@ -243,9 +256,9 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
         }
         return;
     }
-    if (warp > kConsumerThreads / 32) return;
 
     // ==================================== consumer warpgroups ==========================================
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;
     const int g = lane >> 2, tig = lane & 3;
     const int r0 = wg * 64 + (warp & 3) * 16 + g;                 // this thread's tile rows: r0 and r0 + 8
@@ -255,7 +268,8 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     const bool epi_tma = SM::kTmaEpi && p.epi_tma;
     const bool leader = (ctid & 127) == 0;
     uint8_t* my_stage = stage_out + wg * (SM::kStage / 2);
-    uint32_t epi_phase = 0;
+    uint64_t* my_epi_bar = epi_bar + wg * kSlots;
+    uint32_t epi_use = 0;                                         // rounds each slot has served
     constexpr int KS = PREC == 2 ? 2 : 4;                         // k-steps per k-block: 16 bf16 or 8 tf32 each
     using Frag = uint32_t[KS][4];                                 // this thread's A fragments of one k-block (hi or lo)
     // Wait for ring k-block gi, rewrite its B into operand tile set `buf` (CONVB), then load this thread's A fragments of it
@@ -353,7 +367,11 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
             const uint64_t bhi = make_wgmma_desc_sw128(b_addr + ks * 32);
             const uint64_t blo = make_wgmma_desc_sw128(b_addr + (PREC == 2 ? 64 : kTileBBytes) + ks * 32);
             if constexpr (PREC == 2) {
-                if constexpr (BN == 128) {
+                if constexpr (BN == 256) {
+                    wgmma_bf16_n256(acc, hi[ks], bhi, 1);
+                    wgmma_bf16_n256(acc, lo[ks], bhi, 1);
+                    wgmma_bf16_n256(acc, hi[ks], blo, 1);
+                } else if constexpr (BN == 128) {
                     wgmma_bf16_n128(acc, hi[ks], bhi, 1);
                     wgmma_bf16_n128(acc, lo[ks], bhi, 1);
                     wgmma_bf16_n128(acc, hi[ks], blo, 1);
@@ -384,13 +402,20 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
         if (p.atomic_out && t.iters == 0) continue;              // nothing to add
         // origin of this warpgroup's box: channel, then pixel x / y / image / split-K slice
         const int c1 = t.x0 + wg * p.half_x, c2 = t.y0 + wg * p.half_y, c3 = t.img + wg * p.half_b, c4 = t.slice;
-        if (epi_tma && p.epi_load && leader) {
-            // the previous tile's store has read the staging tile: fetch this tile's residual / mask into it now, while
-            // the k-blocks run
-            bulk_wait_read_all();
-            mbar_arrive_expect_tx(&epi_bar[wg], SM::kStage / 2);
+        // Fetch round r's residual / mask boxes into slot r % kSlots of the staging buffers (its previous store has read it).
+        auto fetch_round = [&](int r) {
+            uint8_t* dst = my_stage + (r % kSlots) * (kRound * 8192);
+            mbar_arrive_expect_tx(&my_epi_bar[r % kSlots], kRound * 8192);
 #pragma unroll
-            for (int c = 0; c < BN / 32; ++c) tma_load_5d(my_stage + c * 8192, &mapR, &epi_bar[wg], t.n0 + 32 * c, c1, c2, c3, c4);
+            for (int c = 0; c < kRound; ++c)
+                tma_load_5d(dst + c * 8192, &mapR, &my_epi_bar[r % kSlots], t.n0 + 32 * (r * kRound + c), c1, c2, c3, c4);
+        };
+        if (epi_tma && p.epi_load && leader) {
+            // the previous tile's stores have read the staging buffers: fetch this tile's first rounds of residual / mask
+            // into them now, while the k-blocks run
+            bulk_wait_read_all();
+#pragma unroll
+            for (int r = 0; r < kSlots; ++r) fetch_round(r);
         }
         float acc[NACC];
 #pragma unroll
@@ -443,57 +468,71 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
                     acc[4 * j] += b0; acc[4 * j + 1] += b1; acc[4 * j + 2] += b0; acc[4 * j + 3] += b1;
                 }
             }
-            if (p.epi_load) {
-                mbar_wait(&epi_bar[wg], epi_phase);
-                epi_phase ^= 1;
-            } else {
-                if (leader) bulk_wait_read_all();
-                named_bar_sync(2 + wg, 128);
-            }
-            constexpr int kMB = 8;                                // mask columns groups per batch (registers: 2 x kMB)
+            // The staging buffers hold kRound boxes per slot and kSlots slots: BN = 64 / 128 stage the whole tile as one
+            // round; BN = 256 stages one 32-channel box per round and alternates slots, so that a round is written
+            // while the previous one's store still reads its slot.  With a residual / mask operand, the rounds past the
+            // first kSlots are fetched as their slots drain, behind the tile's k-blocks no longer.
+            constexpr int kMB = 8 < kRound * 4 ? 8 : kRound * 4;  // mask columns groups per batch (registers: 2 x kMB)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = r0 + h * 8, rr = row - 64 * wg;
-                const float* gmask = nullptr;                     // mask beside a TMA-fetched residual: read from global
-                if (p.relu_mask && p.epi_load != 2) {
-                    const int lyt = row / p.tw, lx = row - lyt * p.tw;
-                    const int ib = lyt / p.th, ly = lyt - ib * p.th;
-                    const int y = t.y0 + ly, x = t.x0 + lx, img = t.img + ib;
-                    if ((y < p.Ho) && (x < p.Wo) && (img < p.n_img))
-                        gmask = p.relu_mask + (size_t)((img * p.out_H + y * p.out_sy + p.out_oy) * p.out_W + x * p.out_sx + p.out_ox) * p.ldo;
+            for (int r = 0; r < kRounds; ++r) {                   // unrolled: the accumulators are indexed by r
+                uint8_t* slot = my_stage + (r % kSlots) * (kRound * 8192);
+                if (p.epi_load) {
+                    mbar_wait(&my_epi_bar[r % kSlots], (epi_use + r / kSlots) & 1);
+                } else {
+                    if (leader) bulk_wait_read<kSlots - 1>();     // the store that last read this slot is done with it
+                    named_bar_sync_diverged(2 + wg, 128);         // (the leader's lane may still be in its branch)
                 }
 #pragma unroll
-                for (int j0 = 0; j0 < BN / 8; j0 += kMB) {
-                    float2 mv[kMB];                               // 0 for rows past the output (computed, never stored)
-#pragma unroll
-                    for (int u = 0; u < kMB; ++u) {
-                        const int n = t.n0 + (j0 + u) * 8 + tig * 2;
-                        mv[u] = (gmask && n < p.No) ? *reinterpret_cast<const float2*>(gmask + n) : make_float2(0.f, 0.f);
+                for (int h = 0; h < 2; ++h) {
+                    const int row = r0 + h * 8, rr = row - 64 * wg;
+                    const float* gmask = nullptr;                 // mask beside a TMA-fetched residual: read from global
+                    if (p.relu_mask && p.epi_load != 2) {
+                        const int lyt = row / p.tw, lx = row - lyt * p.tw;
+                        const int ib = lyt / p.th, ly = lyt - ib * p.th;
+                        const int y = t.y0 + ly, x = t.x0 + lx, img = t.img + ib;
+                        if ((y < p.Ho) && (x < p.Wo) && (img < p.n_img))
+                            gmask = p.relu_mask + (size_t)((img * p.out_H + y * p.out_sy + p.out_oy) * p.out_W + x * p.out_sx + p.out_ox) * p.ldo;
                     }
 #pragma unroll
-                    for (int u = 0; u < kMB; ++u) {
-                        const int j = j0 + u, n = t.n0 + j * 8 + tig * 2;
-                        if (n >= p.No) continue;
-                        float2* sp = reinterpret_cast<float2*>(my_stage + (j >> 2) * 8192 + raw_off<false>(rr, (j & 3) * 8 + tig * 2));
-                        float v[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};   // (+ bias; the register path's * 1.f: exact)
-                        if (p.epi_load == 1) { const float2 e = *sp; v[0] += e.x; v[1] += e.y; }
-                        if (p.relu) { v[0] = fmaxf(v[0], 0.f); v[1] = fmaxf(v[1], 0.f); }
-                        if (p.relu_mask) {
-                            const float2 m = p.epi_load == 2 ? *sp : mv[u];
-                            v[0] = m.x > 0.f ? v[0] : 0.f; v[1] = m.y > 0.f ? v[1] : 0.f;
+                    for (int j0 = 0; j0 < kRound * 4; j0 += kMB) {
+                        float2 mv[kMB];                           // 0 for rows past the output (computed, never stored)
+#pragma unroll
+                        for (int u = 0; u < kMB; ++u) {
+                            const int n = t.n0 + (r * kRound * 4 + j0 + u) * 8 + tig * 2;
+                            mv[u] = (gmask && n < p.No) ? *reinterpret_cast<const float2*>(gmask + n) : make_float2(0.f, 0.f);
                         }
-                        if (p.round_out) { v[0] = round_tf32(v[0]); v[1] = round_tf32(v[1]); }
-                        *sp = make_float2(v[0], v[1]);
+#pragma unroll
+                        for (int u = 0; u < kMB; ++u) {
+                            const int jl = j0 + u, j = r * kRound * 4 + jl, n = t.n0 + j * 8 + tig * 2;
+                            if (n >= p.No) continue;
+                            float2* sp = reinterpret_cast<float2*>(slot + (jl >> 2) * 8192 + raw_off<false>(rr, (j & 3) * 8 + tig * 2));
+                            float v[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};   // (+ bias; the register path's * 1.f: exact)
+                            if (p.epi_load == 1) { const float2 e = *sp; v[0] += e.x; v[1] += e.y; }
+                            if (p.relu) { v[0] = fmaxf(v[0], 0.f); v[1] = fmaxf(v[1], 0.f); }
+                            if (p.relu_mask) {
+                                const float2 m = p.epi_load == 2 ? *sp : mv[u];
+                                v[0] = m.x > 0.f ? v[0] : 0.f; v[1] = m.y > 0.f ? v[1] : 0.f;
+                            }
+                            if (p.round_out) { v[0] = round_tf32(v[0]); v[1] = round_tf32(v[1]); }
+                            *sp = make_float2(v[0], v[1]);
+                        }
                     }
                 }
-            }
-            fence_proxy_async_smem();      // generic-proxy writes -> visible to the bulk copy's async-proxy reads
-            named_bar_sync(2 + wg, 128);
-            if (leader) {
+                fence_proxy_async_smem();      // generic-proxy writes -> visible to the bulk copy's async-proxy reads
+                named_bar_sync_diverged(2 + wg, 128);
+                if (leader) {
 #pragma unroll
-                for (int c = 0; c < BN / 32; ++c) tma_store_5d(&mapO, my_stage + c * 8192, t.n0 + 32 * c, c1, c2, c3, c4);
-                bulk_commit();
+                    for (int c = 0; c < kRound; ++c)
+                        tma_store_5d(&mapO, slot + c * 8192, t.n0 + 32 * (r * kRound + c), c1, c2, c3, c4);
+                    bulk_commit();
+                    if (p.epi_load && r + kSlots < kRounds) {
+                        bulk_wait_read_all();
+                        fetch_round(r + kSlots);
+                    }
+                }
+                __syncwarp();                  // the leader's lane rejoins its warp before the next round's barrier
             }
+            epi_use += kRounds / kSlots;
             continue;
         }
         // ---- epilogue: accumulator registers -> fused bias / residual / ReLU / mask / row-scale -> global ------------
@@ -712,9 +751,32 @@ int setup_epi_px(TcParams& p, CUtensorMap* mo, CUtensorMap* mr, size_t off, int 
     return 0;
 }
 
+// Ring depth of the 128 x 256 BF16x3 tile: 4 stages of 48 KB leave 32 KB of staging (two 32-channel boxes per warpgroup).
+constexpr int kWideStages = 4;
+
+// Tile width of a BF16x3 fprop / dgrad launch with N output channels, `m_tiles` row tiles (per split-K slice, `slices`
+// of them) and `kblocks` k-blocks per tile: 256 where N is a multiple of 256, the reduction is long and the wide tiles
+// leave no CTA more work than the 128-wide ones do.  The wide tile's epilogue stages its 256 columns one 32-channel box
+// at a time, so it costs more per tile than the 128-wide one's; only long reductions repay it (H100, 400 W: the 3x3
+// 256 -> 256 convolution at 24 x 80, 72 k-blocks, 12 % faster; 1x1 layers with 2 - 32 k-blocks 2 - 15 % slower).  A wide
+// tile costs per CTA what two 128-wide tiles cost, so it is taken when ceil(T256 / SMs) * 2 <= ceil(T128 / SMs) (3x3
+// 512 -> 512 at 12 x 40, batch 8: 120 tiles at 128 on 132 SMs, one wave; 60 tiles at 256 would double it).  Every output
+// element sees the same wgmmas in the same k order at either width, so the choice does not change the result.
+constexpr int kWideMinKBlocks = 64;
+int pick_bn(int N, int m_tiles, int slices, int kblocks) {
+    const int base = N <= 64 ? 64 : 128;
+    if (N % 256 || kblocks < kWideMinKBlocks) return base;
+    const long long sms = num_sms(), t256 = (long long)m_tiles * (N / 256) * (slices > 0 ? slices : 1);
+    const long long w256 = (t256 + sms - 1) / sms, w128 = (2 * t256 + sms - 1) / sms;
+    return 2 * w256 <= w128 ? 256 : base;
+}
+
 // Launch the fprop / dgrad kernel (K-major B operand) for the arithmetic mode.
 int launch_fwd(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr, const TcParams& p, dim3 grid, int bn, int precision, cudaStream_t stream) {
-    if (precision == 2) return bn == 64 ? launch_tc<64, 6, 0, false, 2>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 2>(ma, mb, mo, mr, p, grid, stream);
+    if (precision == 2) {
+        if (bn == 256) return launch_tc<256, kWideStages, 0, false, 2>(ma, mb, mo, mr, p, grid, stream);
+        return bn == 64 ? launch_tc<64, 6, 0, false, 2>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 2>(ma, mb, mo, mr, p, grid, stream);
+    }
     if (precision == 1) return bn == 64 ? launch_tc<64, 5, 0, false, 1>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 3, 0, false, 1>(ma, mb, mo, mr, p, grid, stream);
     return bn == 64 ? launch_tc<64, 6, 0, false, 0>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 0>(ma, mb, mo, mr, p, grid, stream);
 }
@@ -797,16 +859,17 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
     p.No = Cout; p.ldo = Cout; p.relu = flags & 1; p.round_out = (precision == 0) ? ((flags >> 1) & 1) : 0; p.atomic_out = 0;
     p.bias = bias; p.residual = residual; p.relu_mask = nullptr; p.rowscale = nullptr; p.out = y;
 
-    const int bn = Cout <= 64 ? 64 : 128;
-    dim3 grid((Cout + bn - 1) / bn, n_groups * p.tiles_x * p.tiles_y, 1);
     const long long out_elems = (long long)B * g.Ho * g.Wo * Cout;
     const int slices = ((reinterpret_cast<uintptr_t>(bias) & 15u) == 0)
-                           ? forward_splitk_slices(precision, p.ntaps * p.cblocks, bn, !residual && !p.relu, Cout, out_elems)
+                           ? forward_splitk_slices(precision, p.ntaps * p.cblocks, Cout <= 64 ? 64 : 128, !residual && !p.relu, Cout, out_elems)
                            : 0;
     if (query_ws) {
         *query_ws = sizeof(float) * (size_t)out_elems * slices;
         return 0;
     }
+    const int m_tiles = n_groups * p.tiles_x * p.tiles_y;
+    const int bn = precision == 2 ? pick_bn(Cout, m_tiles, slices, slices > 0 ? 32 : p.ntaps * p.cblocks) : (Cout <= 64 ? 64 : 128);
+    dim3 grid((Cout + bn - 1) / bn, m_tiles, 1);
 
     CUtensorMap ma, mb;
     {   // A: x as (C, W, H, B), box (32, tw*s, th*s, 1), element strides (1, s, s, 1)
@@ -851,7 +914,7 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
             grid.z = slices;
             rc = setup_epi_px(p, &mo, &mr, 0, g.Wo, g.Ho, B, pix_x, pix_y, pix_b, slices);
             if (rc) return rc;
-            rc = launch_fwd(ma, mb, mo, mr, p, grid, 128, precision, stream);
+            rc = launch_fwd(ma, mb, mo, mr, p, grid, bn, precision, stream);
             if (rc) return rc;
             const long long n4 = out_elems / 4;
             splitk_reduce_kernel<<<grid_cap(n4, 256, num_sms() * 8), 256, 0, stream>>>(
@@ -922,7 +985,7 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
                 rc = make_map(&ma, dy, 4, dims, str, box, nullptr);
                 if (rc) return rc;
             }
-            const int bn = (bf && Cin <= 64) ? 64 : 128;
+            const int bn = bf ? pick_bn(Cin, n_groups * p.tiles_x * p.tiles_y, 0, nt * p.cblocks) : 128;
             if (bf) {   // B (K-major): transposed pre-split weights as (64 * k-blocks, Cin, taps); box (64, BN, 1)
                 const uint64_t kb = (uint64_t)p.cblocks;
                 uint64_t dims[3] = {64 * kb, (uint64_t)Cin, (uint64_t)(kh * kw)};

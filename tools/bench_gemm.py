@@ -76,17 +76,29 @@ def pick_tile3(W, H, Bn, n_pix=128):
     return res
 
 
-def fwd_schedule(H, W, Cin, Cout, k, sms):
-    """(tiles per CTA, k-blocks per tile) of a stride-1 fprop launch (B = 8) with Cin in, Cout out; a dgrad of the layer
-    Cin -> Cout is the fprop Cout -> Cin.  Restates the tile walk of conv_forward_impl (no split-K at these shapes)."""
+def pick_bn(N, m_tiles, kblocks, sms, mode):
+    """Tile width of an fprop / dgrad launch with N output columns: restates pick_bn of conv_gemm.cu (BF16x3 only)."""
+    base = 64 if N <= 64 else 128
+    if mode != "bf16x3" or N % 256 or kblocks < 64:
+        return base
+    t = m_tiles * (N // 256)
+    return 256 if 2 * -(-t // sms) <= -(-2 * t // sms) else base
+
+
+def fwd_schedule(H, W, Cin, Cout, k, sms, mode="bf16x3"):
+    """(tiles per CTA, k-blocks per tile, tile width) of a stride-1 fprop launch (B = 8) with Cin in, Cout out; a dgrad
+    of the layer Cin -> Cout is the fprop Cout -> Cin.  Restates the tile walk of conv_forward_impl (no split-K at these
+    shapes)."""
     if k == 1:
         W, H, Bn = B * H * W, 1, 1
     else:
         Bn = B
     tw, th, tb = pick_tile3(W, H, Bn)
     m_tiles = -(-W // tw) * -(-H // th) * -(-Bn // tb)
-    tiles = m_tiles * -(-Cout // (64 if Cout <= 64 else 128))
-    return -(-tiles // min(tiles, sms)), k * k * -(-Cin // 32)
+    kb = k * k * -(-Cin // 32)
+    bn = pick_bn(Cout, m_tiles, kb, sms, mode)
+    tiles = m_tiles * -(-Cout // bn)
+    return -(-tiles // min(tiles, sms)), kb, bn
 
 
 def wgrad_schedule(M, Cin, Cout, sms):
@@ -156,7 +168,8 @@ if "--tile-probe" in sys.argv:
     sys.exit(0)
 
 sms = torch.cuda.get_device_properties(0).multi_processor_count
-print(f"== {card()}; {sms} SMs.  clk/kb = SM clocks per k-block of 32 (time x SM clock / (tiles per CTA x k-blocks per tile))")
+print(f"== {card()}; {sms} SMs.  clk/kb = SM clocks per k-block of 32 (time x SM clock / (tiles per CTA x k-blocks per tile)); "
+      "n = tile width (a 256-wide tile does twice a 128-wide one's work per k-block)")
 for mode in tuple(os.environ["MDB_MODES"].split(",")) if os.environ.get("MDB_MODES") else (("tf32x3",) if os.environ.get("MDB_ONLY_X3") else ("bf16x3", "tf32x3", "tf32")):
     tc.set_precision(mode)
     print(f"== {mode}")
@@ -177,8 +190,9 @@ for mode in tuple(os.environ["MDB_MODES"].split(",")) if os.environ.get("MDB_MOD
         t_w = timeit(lambda: tc.conv2d_wgrad(dy, x, None, k, k, s, pad))
         mhz = mhz or sm_mhz()   # sampled once per mode, right after the first shape's timings
         clk = lambda t, sched: f"{t * mhz / (sched[0] * sched[1]):5.0f}" if mhz else "  n/a"
+        sf, sd = fwd_schedule(H, W, Cin, Cout, k, sms, mode), fwd_schedule(H, W, Cout, Cin, k, sms, mode)
         print(f"{name:34s} fwd {t_f:7.1f} us ({flop / t_f / 1e6:6.1f} TF/s, {byt / t_f / 1e3:6.0f} GB/s, "
-              f"{clk(t_f, fwd_schedule(H, W, Cin, Cout, k, sms))} clk/kb)  fwd+res {t_fr:7.1f}  "
-              f"dgrad+mask {t_d:7.1f} ({flop / t_d / 1e6:6.1f} TF/s, {clk(t_d, fwd_schedule(H, W, Cout, Cin, k, sms))} clk/kb)  "
+              f"{clk(t_f, sf)} clk/kb, n {sf[2]:3d})  fwd+res {t_fr:7.1f}  "
+              f"dgrad+mask {t_d:7.1f} ({flop / t_d / 1e6:6.1f} TF/s, {clk(t_d, sd)} clk/kb, n {sd[2]:3d})  "
               f"wgrad {t_w:7.1f} ({flop / t_w / 1e6:6.1f} TF/s)")
     print(f"   SM clock sampled: {mhz} MHz")
