@@ -111,6 +111,13 @@ int mdb_msda_fused_backward_f32(const float* value, const int64_t* spatial_shape
  * with B=1, H=1, W=M, Cin=K, Cout=N, kh=kw=1, stride=1, pad=0 (w itself is already "packed").
  * Supported: kh=kw in {1,3}, stride in {1,2}, Cin%4==0, 16-byte aligned pointers; Cout%4==0 for dgrad / wgrad (the
  * forward writes any Cout, e.g. the 3-class / 81-bin head widths of monodetr.py:102-117); outputs below 2^31 elements.
+ * The *_dilated entry points take a dilation d >= 1 after pad (torch.nn.Conv2d's dilation: taps d pixels apart, output
+ * size (H + 2*pad - d*(kh-1) - 1)/stride + 1); d > 1 requires kh == kw == 3 and stride 1, and the weight gradient also
+ * pad % d == 0 (the dilated C5 stage of torchvision's ResNets, backbone.py:100-106: pad == d); anything else returns
+ * MDB_EUNSUPPORTED.  A dilated launch runs the same
+ * tiles, k order and split-K decision as the undilated one of the same shape, so every statement below holds for it too
+ * (the dilated weight gradient is the sum of d*d undilated ones over the dilation's pixel lattices, launched in turn);
+ * with d == 1 they are the plain entry points.
  * Forward and dgrad store their output with TMA (staged in shared memory, residual or mask fetched by TMA) when the output
  * width is a multiple of 4 and y / dx, residual and relu_mask are 16-byte aligned, and from registers otherwise (e.g. the
  * odd head widths); both give the same bits.
@@ -167,6 +174,24 @@ int mdb_conv2d_wgrad_f32(const float* dy, const float* x, const float* rowscale 
 int mdb_conv2d_wgrad_bias_f32(const float* dy, const float* x, const float* rowscale /*[Cout]|NULL*/, float* dw_packed,
                               float* db /*[Cout]|NULL*/, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride,
                               int pad, int accumulate, void* stream);
+/* Dilated twins of the forward / dgrad / wgrad / workspace calls above (see "Supported"): `dilation` follows `pad`. */
+int mdb_conv2d_forward_dilated_bf16x3(const float* x, const void* w_split, const float* bias, const float* residual, float* y,
+                                      int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                      int flags, void* stream);
+int mdb_conv2d_forward_dilated_f32(const float* x, const float* w_packed, const float* bias, const float* residual, float* y,
+                                   int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                   int flags, void* stream);
+int mdb_conv2d_dgrad_dilated_bf16x3(const float* dy, const void* w_split_t, const float* residual, const float* relu_mask,
+                                    float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                    int dilation, int flags, void* stream);
+int mdb_conv2d_dgrad_dilated_f32(const float* dy, const float* w_packed, const float* residual, const float* relu_mask,
+                                 float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                 int dilation, int flags, void* stream);
+int mdb_conv2d_wgrad_bias_dilated_f32(const float* dy, const float* x, const float* rowscale /*[Cout]|NULL*/, float* dw_packed,
+                                      float* db /*[Cout]|NULL*/, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride,
+                                      int pad, int dilation, int accumulate, void* stream);
+long long mdb_conv2d_forward_workspace_bytes_dilated(int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                                     int dilation, int flags, int has_residual, int split_weights);
 /* w_packed[t][o][i] = w_oihw[o][i][t] * (scale ? scale[o] : 1), rounded to nearest TF32 in precision mode 0
  * (FrozenBatchNorm fold, backbone.py:54-64) */
 int mdb_pack_conv_weight_f32(const float* w_oihw, const float* scale, float* w_packed, int O, int I, int taps,

@@ -34,6 +34,12 @@ SIGNATURES = {
     "mdb_conv2d_forward_bf16x3": [_PTR] * 5 + [c_int] * 10 + [_PTR],
     "mdb_conv2d_dgrad_bf16x3": [_PTR] * 5 + [c_int] * 10 + [_PTR],
     "mdb_conv2d_forward_workspace_bytes": [c_int] * 12,
+    "mdb_conv2d_forward_dilated_f32": [_PTR] * 5 + [c_int] * 11 + [_PTR],
+    "mdb_conv2d_forward_dilated_bf16x3": [_PTR] * 5 + [c_int] * 11 + [_PTR],
+    "mdb_conv2d_dgrad_dilated_f32": [_PTR] * 5 + [c_int] * 11 + [_PTR],
+    "mdb_conv2d_dgrad_dilated_bf16x3": [_PTR] * 5 + [c_int] * 11 + [_PTR],
+    "mdb_conv2d_wgrad_bias_dilated_f32": [_PTR] * 5 + [c_int] * 11 + [_PTR],
+    "mdb_conv2d_forward_workspace_bytes_dilated": [c_int] * 13,
     "mdb_set_workspace": [_PTR, ctypes.c_ulonglong],
     "mdb_pack_gemm_weights_bf16x3": [c_int] + [_PTR] * 7 + [c_int, _PTR],
     "mdb_conv2d_dgrad_f32": [_PTR] * 5 + [c_int] * 10 + [_PTR],
@@ -88,6 +94,7 @@ SIGNATURES = {
     "mdb_kitti_compact_dets": [_PTR] * 3 + [c_int] * 2 + [_PTR] * 3,
 }
 _RESTYPES = {"mdb_error_string": ctypes.c_char_p, "mdb_conv2d_forward_workspace_bytes": ctypes.c_longlong,
+             "mdb_conv2d_forward_workspace_bytes_dilated": ctypes.c_longlong,
              "mdb_kitti_eval_workspace_bytes": ctypes.c_longlong}
 
 

@@ -1,7 +1,8 @@
-"""ResNet-50 backbone on the sm_90a kernels -- host-side mirror of the reference's
+"""ResNet backbones on the sm_90a kernels -- host-side mirror of the reference's
 lib/models/monodetr/backbone.py (FrozenBatchNorm2d :27-64, BackboneBase :67-90, Backbone :93-108, Joiner
-:111-126, build_backbone :129-135) with torchvision's resnet50 (v1.5, stride on the 3x3) restated as parameter
-containers with the same state_dict keys (`backbone.0.body.*`).
+:111-126, build_backbone :129-135) with torchvision's bottleneck ResNets (resnet50 / 101 / 152, v1.5: stride on the 3x3;
+optionally with layer4's stride replaced by dilation 2, the "DC5" variant) restated as parameter containers with the same
+state_dict keys (`backbone.0.body.*`).
 
 Execution is ONE hand-scheduled autograd Function (no cuDNN, no per-layer autograd nodes):
   * conv1 7x7/2 + FrozenBN + ReLU and max-pool: dedicated forward-only kernels (conv1/layer1 are frozen, :71-73);
@@ -20,7 +21,9 @@ from torch.autograd.function import once_differentiable
 from . import _lib, tc
 from .position_encoding import build_position_encoding
 
-_STAGES = [("layer1", 64, 3, 1), ("layer2", 128, 4, 2), ("layer3", 256, 6, 2), ("layer4", 512, 3, 2)]
+# (stage, planes, stride) of torchvision's ResNet, and the blocks per stage of each bottleneck depth it builds
+_STAGES = [("layer1", 64, 1), ("layer2", 128, 2), ("layer3", 256, 2), ("layer4", 512, 2)]
+RESNET_DEPTHS = {"resnet50": (3, 4, 6, 3), "resnet101": (3, 4, 23, 3), "resnet152": (3, 8, 36, 3)}
 
 
 class FrozenBatchNorm2d(nn.Module):
@@ -43,8 +46,8 @@ class FrozenBatchNorm2d(nn.Module):
         return scale.contiguous(), (self.bias - self.running_mean * scale).contiguous()
 
 
-def _conv(cin, cout, k, stride=1):
-    m = nn.Conv2d(cin, cout, k, stride=stride, padding=k // 2, bias=False)     # parameter container only
+def _conv(cin, cout, k, stride=1, dilation=1):
+    m = nn.Conv2d(cin, cout, k, stride=stride, padding=dilation * (k // 2), dilation=dilation, bias=False)   # parameter container only
     nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
     return m
 
@@ -52,11 +55,11 @@ def _conv(cin, cout, k, stride=1):
 class Bottleneck(nn.Module):
     expansion = 4
 
-    def __init__(self, inplanes, planes, stride, downsample):
+    def __init__(self, inplanes, planes, stride, downsample, dilation=1):
         super().__init__()
         self.conv1 = _conv(inplanes, planes, 1)
         self.bn1 = FrozenBatchNorm2d(planes)
-        self.conv2 = _conv(planes, planes, 3, stride)
+        self.conv2 = _conv(planes, planes, 3, stride, dilation)
         self.bn2 = FrozenBatchNorm2d(planes)
         self.conv3 = _conv(planes, planes * 4, 1)
         self.bn3 = FrozenBatchNorm2d(planes * 4)
@@ -64,26 +67,34 @@ class Bottleneck(nn.Module):
         if downsample:
             self.downsample = nn.Sequential(_conv(inplanes, planes * 4, 1, stride), FrozenBatchNorm2d(planes * 4))
         self.stride = stride
+        self.dilation = dilation
 
 
-class ResNet50Body(nn.Module):
-    """Parameter tree with torchvision's names: conv1, bn1, layer1..layer4 (what IntermediateLayerGetter keeps)."""
+class ResNetBody(nn.Module):
+    """Parameter tree with torchvision's names: conv1, bn1, layer1..layer4 (what IntermediateLayerGetter keeps).
+    `depths` = blocks per stage (RESNET_DEPTHS); `dilate_c5` = torchvision's replace_stride_with_dilation=[False, False, True]:
+    layer4's block 0 keeps dilation 1 with stride 1 (its 1x1 downsample too), blocks 1.. are 3x3 with dilation 2 / padding 2."""
 
-    def __init__(self):
+    def __init__(self, depths=RESNET_DEPTHS["resnet50"], dilate_c5=False):
         super().__init__()
         self.conv1 = nn.Conv2d(3, 64, 7, stride=2, padding=3, bias=False)
         nn.init.kaiming_normal_(self.conv1.weight, mode="fan_out", nonlinearity="relu")
         self.bn1 = FrozenBatchNorm2d(64)
         inplanes = 64
-        for name, planes, blocks, stride in _STAGES:
+        for (name, planes, stride), blocks in zip(_STAGES, depths):
+            dilated = dilate_c5 and name == "layer4"
             layers = []
             for i in range(blocks):
-                layers.append(Bottleneck(inplanes, planes, stride if i == 0 else 1, downsample=(i == 0)))
+                if dilated:      # (stride, dilation): torchvision's _make_layer with dilate=True
+                    blk_stride, blk_dil = 1, (1 if i == 0 else stride)
+                else:
+                    blk_stride, blk_dil = (stride if i == 0 else 1), 1
+                layers.append(Bottleneck(inplanes, planes, blk_stride, downsample=(i == 0), dilation=blk_dil))
                 inplanes = planes * 4
             setattr(self, name, nn.Sequential(*layers))
 
     def blocks(self):
-        for name, _, _, _ in _STAGES:
+        for name, _, _ in _STAGES:
             for blk in getattr(self, name):
                 yield name, blk
 
@@ -118,12 +129,12 @@ class _ResNetFn(Function):
         else:
             all_wp = [None] + tc.pack_weights_multi(list(weights[1:nconv]), list(scales[1:nconv]))
         ci = 1
-        for bi, (stage, stride, has_ds, trainable) in enumerate(meta["blocks"]):
+        for bi, (stage, stride, dil, has_ds, trainable) in enumerate(meta["blocks"]):
             idx = [ci, ci + 1, ci + 2] + ([ci + 3] if has_ds else [])
             ci += len(idx)
             wp = [all_wp[j] for j in idx]
             o1 = tc.conv2d_forward(x, wp[0], shifts[idx[0]], None, 1, 1, 1, 0, relu=True, round_out=True)
-            o2 = tc.conv2d_forward(o1, wp[1], shifts[idx[1]], None, 3, 3, stride, 1, relu=True, round_out=True)
+            o2 = tc.conv2d_forward(o1, wp[1], shifts[idx[1]], None, 3, 3, stride, dil, relu=True, round_out=True, dilation=dil)
             if has_ds:
                 idn = tc.conv2d_forward(x, wp[3], shifts[idx[3]], None, 1, 1, stride, 0, relu=False)
             else:
@@ -146,8 +157,8 @@ class _ResNetFn(Function):
     def backward(ctx, *gfeats):
         meta = ctx.meta
         nconv = meta["nconv"]
-        blocks = [b for b in meta["blocks"] if b[3]]                 # trainable blocks, in forward order
-        ends = [e for b, e in zip(meta["blocks"], meta["stage_end"]) if b[3]]
+        blocks = [b for b in meta["blocks"] if b[4]]                 # trainable blocks, in forward order
+        ends = [e for b, e in zip(meta["blocks"], meta["stage_end"]) if b[4]]
         conv_idx = meta["train_conv_idx"]                            # per trainable block: indices into weights
         grads = [None] * (3 * nconv)
         # which feature gradient enters after which trainable block
@@ -160,7 +171,7 @@ class _ResNetFn(Function):
         g = None                                                      # grad wrt block output, already ReLU-masked
         pending = []                                                  # 3x3 weight gradients still in packed layout
         for k in range(len(blocks) - 1, -1, -1):
-            stage, stride, has_ds, _ = blocks[k]
+            stage, stride, dil, has_ds, _ = blocks[k]
             x, o1, o2, out = ctx.saved[k]
             wp = ctx.packed[k]
             idx = conv_idx[k]
@@ -170,9 +181,9 @@ class _ResNetFn(Function):
             # conv3
             grads[idx[2]] = tc.conv2d_wgrad(g, o2, sc[2], 1, 1, 1, 0).view_as(_w(ctx, idx[2]))
             g2 = tc.conv2d_dgrad(g, wp[2], o2.shape, None, o2, 1, 1, 1, 0, round_out=True)
-            # conv2 (3x3, maybe strided)
-            pending.append((idx[1], tc.conv2d_wgrad(g2, o1, sc[1], 3, 3, stride, 1)))   # 3x3: [tap][O][I] -> OIHW at the end
-            g1 = tc.conv2d_dgrad(g2, wp[1], o1.shape, None, o1, 3, 3, stride, 1, round_out=True)
+            # conv2 (3x3, maybe strided or dilated; padding = dilation)
+            pending.append((idx[1], tc.conv2d_wgrad(g2, o1, sc[1], 3, 3, stride, dil, dilation=dil)))   # [tap][O][I] -> OIHW at the end
+            g1 = tc.conv2d_dgrad(g2, wp[1], o1.shape, None, o1, 3, 3, stride, dil, round_out=True, dilation=dil)
             # conv1
             grads[idx[0]] = tc.conv2d_wgrad(g1, x, sc[0], 1, 1, 1, 0).view_as(_w(ctx, idx[0]))
             if has_ds:
@@ -251,7 +262,7 @@ class BackboneBase(nn.Module):
         for i, (name, blk) in enumerate(self.body.blocks()):
             has_ds = blk.downsample is not None
             trainable = blk.conv1.weight.requires_grad
-            blocks.append((name, blk.stride, has_ds, trainable))
+            blocks.append((name, blk.stride, blk.dilation, has_ds, trainable))
             stage_end.append(i + 1 == len(names) or names[i + 1] != name)
             idx = [ci, ci + 1, ci + 2] + ([ci + 3] if has_ds else [])
             if trainable:
@@ -264,12 +275,18 @@ class BackboneBase(nn.Module):
 
 
 class Backbone(BackboneBase):
-    """ResNet backbone with frozen BatchNorm (reference :93-108; only resnet50 without dilation is implemented)."""
+    """ResNet backbone with frozen BatchNorm (reference :93-108): torchvision's bottleneck ResNets with plain convolutions
+    (resnet50 / resnet101 / resnet152), each with or without the dilated C5 stage."""
 
     def __init__(self, name: str, train_backbone: bool, return_interm_layers: bool, dilation: bool):
-        if name != "resnet50" or dilation:
-            raise NotImplementedError("monodetr_b200 implements the configs/monodetr.yaml backbone: resnet50, dilation False")
-        super().__init__(ResNet50Body(), train_backbone, return_interm_layers)
+        if name not in RESNET_DEPTHS:
+            # resnet18 / 34 (basic blocks: the reference asserts against them) and the grouped / widened convolutions of
+            # ResNeXt and wide ResNets have no kernels here
+            raise NotImplementedError(f"monodetr_b200 backbone {name!r}: supported are {', '.join(RESNET_DEPTHS)}, "
+                                      "each with dilation False or True")
+        super().__init__(ResNetBody(RESNET_DEPTHS[name], bool(dilation)), train_backbone, return_interm_layers)
+        if dilation:
+            self.strides[-1] = self.strides[-1] // 2
 
 
 class Joiner(nn.Sequential):

@@ -782,12 +782,22 @@ int launch_fwd(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& 
 }
 
 struct ConvGeom {
-    int B, H, W, Cin, Cout, kh, kw, stride, pad, Ho, Wo;
+    int B, H, W, Cin, Cout, kh, kw, stride, pad, dil, Ho, Wo;
 };
+
+// Output size of a convolution (torch.nn.Conv2d's formula).
+int conv_out(int n, int k, int stride, int pad, int dil) { return (n + 2 * pad - dil * (k - 1) - 1) / stride + 1; }
+
+ConvGeom make_geom(int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dil) {
+    return ConvGeom{B, H, W, Cin, Cout, kh, kw, stride, pad, dil, conv_out(H, kh, stride, pad, dil), conv_out(W, kw, stride, pad, dil)};
+}
 
 int check_geom(const ConvGeom& g, bool forward = false) {
     if (g.B <= 0 || g.H <= 0 || g.W <= 0 || g.Cin <= 0 || g.Cout <= 0) return MDB_EINVAL;
     if (g.kh != g.kw || (g.kh != 1 && g.kh != 3) || (g.stride != 1 && g.stride != 2)) return MDB_EUNSUPPORTED;
+    // Dilation only changes the taps' box offsets; it is supported where ResNet's DC5 stage uses it: 3x3, stride 1.  (A
+    // strided dilated dgrad would need per-parity tap sets of a different shape.)
+    if (g.dil < 1 || (g.dil > 1 && (g.kh != 3 || g.stride != 1))) return MDB_EUNSUPPORTED;
     // TMA needs 16-byte row pitches on every operand it reads: Cin always; Cout only where dy / the output map is an
     // operand (dgrad, wgrad).  The forward epilogue writes ragged Cout with scalar stores.
     if (g.Cin % 4 || (!forward && g.Cout % 4)) return MDB_EUNSUPPORTED;
@@ -825,10 +835,10 @@ int forward_splitk_slices(int precision, int kblocks, int bn, bool plain_epilogu
 // y[B,Ho,Wo,Cout] = act( conv(x[B,H,W,Cin], w) + bias + residual );  w = fp32 packed [kh*kw][Cout][Cin] (bf == false)
 // or the pre-split bf16 form [kh*kw][Cout][ceil(Cin/32)][hi 32 | lo 32] (bf == true, precision mode 2).
 int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float* bias, const float* residual, float* y,
-                      int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int flags,
+                      int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dil, int flags,
                       void* stream_, size_t* query_ws = nullptr /* non-null: only report the scratch bytes this call needs */) {
     const int precision = bf ? 2 : (g_precision == 2 ? 1 : g_precision);   // fp32 weights in bf16x3 mode: 3xTF32
-    ConvGeom g{B, H, W, Cin, Cout, kh, kw, stride, pad, (H + 2 * pad - kh) / stride + 1, (W + 2 * pad - kw) / stride + 1};
+    ConvGeom g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dil);
     int rc = check_geom(g, true);
     if (rc) return rc;
     if (!query_ws && (!x || !w_packed || !y)) return MDB_EINVAL;
@@ -836,7 +846,7 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     if (kh == 1 && stride == 1 && pad == 0) {     // pointwise: the batch of images is one long row of pixels (no tile waste)
         W = B * H * W; H = 1; B = 1;
-        g = ConvGeom{B, H, W, Cin, Cout, kh, kw, stride, pad, H, W};
+        g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dil);
     }
     TcParams p;
     memset(&p, 0, sizeof(p));
@@ -853,7 +863,7 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
     for (int ky = 0; ky < kh; ++ky)
         for (int kx = 0; kx < kw; ++kx) {
             const int t = ky * kw + kx;
-            p.tap_dy[t] = ky - pad; p.tap_dx[t] = kx - pad; p.tap_w[t] = t;
+            p.tap_dy[t] = ky * dil - pad; p.tap_dx[t] = kx * dil - pad; p.tap_w[t] = t;
         }
     p.wg_taps = 1; p.wg_kw = 1;
     p.No = Cout; p.ldo = Cout; p.relu = flags & 1; p.round_out = (precision == 0) ? ((flags >> 1) & 1) : 0; p.atomic_out = 0;
@@ -930,10 +940,10 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
 // dx[B,H,W,Cin] = (conv_transpose(dy[B,Ho,Wo,Cout], w) + residual) * (relu_mask > 0);  w = fp32 packed [taps][Cout][Cin]
 // (read MN-major) or, bf == true, the pre-split TRANSPOSED bf16 form [taps][Cin][ceil(Cout/32)][hi 32 | lo 32] (K-major).
 int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float* residual, const float* relu_mask,
-                    float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                    float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dil,
                     int flags, void* stream_) {
     const int precision = bf ? 2 : (g_precision == 2 ? 1 : g_precision);
-    ConvGeom g{B, H, W, Cin, Cout, kh, kw, stride, pad, (H + 2 * pad - kh) / stride + 1, (W + 2 * pad - kw) / stride + 1};
+    ConvGeom g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dil);
     int rc = check_geom(g);
     if (rc) return rc;
     if (!dy || !w_packed || !dx) return MDB_EINVAL;
@@ -941,11 +951,12 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     if (kh == 1 && stride == 1 && pad == 0) {     // pointwise: one long row of pixels
         W = B * H * W; H = 1; B = 1;
-        g = ConvGeom{B, H, W, Cin, Cout, kh, kw, stride, pad, H, W};
+        g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dil);
     }
-    // dx[y,x] = sum_{ky,kx} dy[(y+pad-ky)/s, (x+pad-kx)/s] * W[ky,kx]  where the division is exact.
+    // dx[y,x] = sum_{ky,kx} dy[(y+pad-ky*d)/s, (x+pad-kx*d)/s] * W[ky,kx]  where the division is exact.
     // Per output parity class (py,px) (only one class for s == 1) the contributing taps are fixed and the
-    // dy access is a unit-stride shifted box: oy = (y + pad - ky)/s = j + (py + pad - ky)/s  for y = s*j + py.
+    // dy access is a unit-stride shifted box: oy = (y + pad - ky*d)/s = j + (py + pad - ky*d)/s  for y = s*j + py.
+    // (d > 1 only with s == 1: one class, tap offsets pad - ky*d.)
     for (int py = 0; py < stride; ++py)
         for (int px = 0; px < stride; ++px) {
             TcParams p;
@@ -963,12 +974,12 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
             p.cblocks = (Cout + BK - 1) / BK;
             int nt = 0;
             for (int ky = 0; ky < kh; ++ky) {
-                if ((py + pad - ky) % stride) continue;
+                if ((py + pad - ky * dil) % stride) continue;
                 for (int kx = 0; kx < kw; ++kx) {
-                    if ((px + pad - kx) % stride) continue;
+                    if ((px + pad - kx * dil) % stride) continue;
                     // floor division is exact here (numerator divisible by stride; may be negative)
-                    p.tap_dy[nt] = (py + pad - ky) / stride;
-                    p.tap_dx[nt] = (px + pad - kx) / stride;
+                    p.tap_dy[nt] = (py + pad - ky * dil) / stride;
+                    p.tap_dx[nt] = (px + pad - kx * dil) / stride;
                     p.tap_w[nt] = ky * kw + kx;
                     ++nt;
                 }
@@ -1025,20 +1036,34 @@ extern "C" {
 int mdb_conv2d_forward_f32(const float* x, const float* w_packed, const float* bias, const float* residual, float* y,
                            int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int flags,
                            void* stream) {
-    return conv_forward_impl(x, w_packed, false, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, flags, stream);
+    return conv_forward_impl(x, w_packed, false, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, 1, flags, stream);
+}
+int mdb_conv2d_forward_dilated_f32(const float* x, const float* w_packed, const float* bias, const float* residual, float* y,
+                                   int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                   int flags, void* stream) {
+    return conv_forward_impl(x, w_packed, false, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags, stream);
 }
 int mdb_conv2d_forward_bf16x3(const float* x, const void* w_split, const float* bias, const float* residual, float* y,
                               int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int flags,
                               void* stream) {
-    return conv_forward_impl(x, w_split, true, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, flags, stream);
+    return conv_forward_impl(x, w_split, true, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, 1, flags, stream);
 }
-long long mdb_conv2d_forward_workspace_bytes(int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
-                                             int flags, int has_residual, int split_weights) {
+int mdb_conv2d_forward_dilated_bf16x3(const float* x, const void* w_split, const float* bias, const float* residual, float* y,
+                                      int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                      int flags, void* stream) {
+    return conv_forward_impl(x, w_split, true, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags, stream);
+}
+long long mdb_conv2d_forward_workspace_bytes_dilated(int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                                     int dilation, int flags, int has_residual, int split_weights) {
     size_t bytes = 0;
     const float* res = has_residual ? reinterpret_cast<const float*>(16) : nullptr;
     const int rc = conv_forward_impl(nullptr, nullptr, split_weights != 0, nullptr, res, nullptr, B, H, W, Cin, Cout, kh, kw, stride,
-                                     pad, flags, nullptr, &bytes);
+                                     pad, dilation, flags, nullptr, &bytes);
     return rc ? (long long)rc : (long long)bytes;
+}
+long long mdb_conv2d_forward_workspace_bytes(int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                             int flags, int has_residual, int split_weights) {
+    return mdb_conv2d_forward_workspace_bytes_dilated(B, H, W, Cin, Cout, kh, kw, stride, pad, 1, flags, has_residual, split_weights);
 }
 int mdb_set_workspace(void* buf, unsigned long long bytes) {
     DeviceState& d = g_dev[current_device()];
@@ -1049,12 +1074,24 @@ int mdb_set_workspace(void* buf, unsigned long long bytes) {
 int mdb_conv2d_dgrad_f32(const float* dy, const float* w_packed, const float* residual, const float* relu_mask,
                          float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
                          int flags, void* stream) {
-    return conv_dgrad_impl(dy, w_packed, false, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, flags, stream);
+    return conv_dgrad_impl(dy, w_packed, false, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, 1, flags, stream);
+}
+int mdb_conv2d_dgrad_dilated_f32(const float* dy, const float* w_packed, const float* residual, const float* relu_mask,
+                                 float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                 int dilation, int flags, void* stream) {
+    return conv_dgrad_impl(dy, w_packed, false, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags,
+                           stream);
 }
 int mdb_conv2d_dgrad_bf16x3(const float* dy, const void* w_split_t, const float* residual, const float* relu_mask,
                             float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
                             int flags, void* stream) {
-    return conv_dgrad_impl(dy, w_split_t, true, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, flags, stream);
+    return conv_dgrad_impl(dy, w_split_t, true, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, 1, flags, stream);
+}
+int mdb_conv2d_dgrad_dilated_bf16x3(const float* dy, const void* w_split_t, const float* residual, const float* relu_mask,
+                                    float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                    int dilation, int flags, void* stream) {
+    return conv_dgrad_impl(dy, w_split_t, true, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags,
+                           stream);
 }
 
 // dw_packed[tap][Cout][Cin] (+)= rowscale[co] * sum_{b,oy,ox} dy[b,oy,ox,co] * x[b, oy*s+ky-pad, ox*s+kx-pad, ci]
@@ -1067,29 +1104,26 @@ int mdb_conv2d_wgrad_f32(const float* dy, const float* x, const float* rowscale,
 // Same, plus db[Cout] (+)= sum over pixels of dy (the bias gradient, by the column-sum kernel).
 int mdb_conv2d_wgrad_bias_f32(const float* dy, const float* x, const float* rowscale, float* dw_packed, float* db, int B, int H,
                               int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int accumulate, void* stream_) {
-    ConvGeom g{B, H, W, Cin, Cout, kh, kw, stride, pad, (H + 2 * pad - kh) / stride + 1, (W + 2 * pad - kw) / stride + 1};
-    int rc = check_geom(g);
-    if (rc) return rc;
-    if (!dy || !x || !dw_packed) return MDB_EINVAL;
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    if (kh == 1 && stride == 1 && pad == 0) {     // pointwise: one long row of pixels (full 32-pixel reduction tiles)
-        W = B * H * W; H = 1; B = 1;
-        g = ConvGeom{B, H, W, Cin, Cout, kh, kw, stride, pad, H, W};
-    }
+    return mdb_conv2d_wgrad_bias_dilated_f32(dy, x, rowscale, dw_packed, db, B, H, W, Cin, Cout, kh, kw, stride, pad, 1, accumulate,
+                                             stream_);
+}
+
+}  // extern "C"
+
+namespace {
+
+// One weight-gradient launch of an undilated convolution between dy, a Wo x Ho pixel grid with pixel strides (dsx, dsy, dsb)
+// elements, and x, a W x H grid with pixel strides (xsx, xsy, xsb): the whole tensors, or one lattice class of a dilated
+// convolution (below).  Accumulates into dw_packed (zero-filled by the caller) with the kernel's vector reds.
+int wgrad_launch(const float* dy, const float* x, const float* rowscale, float* dw_packed, int B, int Cin, int Cout, int kh,
+                 int kw, int stride, int pad, int Wo, int Ho, uint64_t dsx, uint64_t dsy, uint64_t dsb, int W, int H, uint64_t xsx,
+                 uint64_t xsy, uint64_t xsb, cudaStream_t stream) {
     const int taps = kh * kw;
-    if (!accumulate) {
-        cudaError_t e = cudaMemsetAsync(dw_packed, 0, sizeof(float) * (size_t)taps * Cout * Cin, stream);
-        if (e != cudaSuccess) return (int)e;
-    }
-    if (db) {
-        rc = mdb_colsum_f32(dy, db, (long long)B * g.Ho * g.Wo, Cout, accumulate, stream_);
-        if (rc) return rc;
-    }
     TcParams p;
     memset(&p, 0, sizeof(p));
-    pick_tile(g.Wo, g.Ho, 32, &p.rtw, &p.rth);
-    p.rtiles_x = (g.Wo + p.rtw - 1) / p.rtw;
-    p.rtiles_y = (g.Ho + p.rth - 1) / p.rth;
+    pick_tile(Wo, Ho, 32, &p.rtw, &p.rth);
+    p.rtiles_x = (Wo + p.rtw - 1) / p.rtw;
+    p.rtiles_y = (Ho + p.rth - 1) / p.rth;
     p.n_img = B;
     const int total_red = B * p.rtiles_x * p.rtiles_y;
     const int bn = 128;
@@ -1113,16 +1147,17 @@ int mdb_conv2d_wgrad_bias_f32(const float* dy, const float* x, const float* rows
     p.out = dw_packed;
 
     CUtensorMap ma, mb;
+    int rc;
     {   // A (MN-major): dy as (Cout, Wo, Ho, B); box = 32 channels x (rtw x rth) reduction pixels
-        uint64_t dims[4] = {(uint64_t)Cout, (uint64_t)g.Wo, (uint64_t)g.Ho, (uint64_t)B};
-        uint64_t str[4] = {1, (uint64_t)Cout, (uint64_t)g.Wo * Cout, (uint64_t)g.Ho * g.Wo * Cout};
+        uint64_t dims[4] = {(uint64_t)Cout, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B};
+        uint64_t str[4] = {1, dsx, dsy, dsb};
         uint32_t box[4] = {32, (uint32_t)p.rtw, (uint32_t)p.rth, 1};
         rc = make_map(&ma, dy, 4, dims, str, box, nullptr);
         if (rc) return rc;
     }
     {   // B (MN-major): x as (Cin, W, H, B) with element strides s
         uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-        uint64_t str[4] = {1, (uint64_t)Cin, (uint64_t)W * Cin, (uint64_t)H * W * Cin};
+        uint64_t str[4] = {1, xsx, xsy, xsb};
         uint32_t box[4] = {32, (uint32_t)(p.rtw * stride), (uint32_t)(p.rth * stride), 1};
         uint32_t es[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
         rc = make_map(&mb, x, 4, dims, str, box, es);
@@ -1134,10 +1169,55 @@ int mdb_conv2d_wgrad_bias_f32(const float* dy, const float* x, const float* rows
     memset(&mo, 0, sizeof(mo));
     memset(&mr, 0, sizeof(mr));
     dim3 grid((Cin + bn - 1) / bn, (Cout + BM - 1) / BM, taps * splits);
-    rc = g_precision == 2 ? launch_tc<128, 4, 1, true, 2>(ma, mb, mo, mr, p, grid, stream)
-         : g_precision == 1 ? launch_tc<128, 4, 1, true, 1>(ma, mb, mo, mr, p, grid, stream)
-                            : launch_tc<128, 5, 1, true, 0>(ma, mb, mo, mr, p, grid, stream);
+    return g_precision == 2 ? launch_tc<128, 4, 1, true, 2>(ma, mb, mo, mr, p, grid, stream)
+           : g_precision == 1 ? launch_tc<128, 4, 1, true, 1>(ma, mb, mo, mr, p, grid, stream)
+                              : launch_tc<128, 5, 1, true, 0>(ma, mb, mo, mr, p, grid, stream);
+}
+
+}  // namespace
+
+extern "C" {
+
+// Same with the taps `dilation` pixels apart: x[b, oy*s + ky*d - pad, ox*s + kx*d - pad, ci].  d > 1 (stride 1) also needs
+// pad % d == 0: output pixel (d*j + py, d*i + px) then reads x at (d*(j + ky - pad/d) + py, d*(i + kx - pad/d) + px), so the
+// dilated weight gradient is the sum over the d*d lattice classes (py, px) of UNDILATED ones with padding pad/d between
+// the class's pixels of dy and of x (pixel strides d).  The classes are launched one after another into the same dw (the
+// kernel adds its partial sums anyway; in reproducible mode each launch has one writer per element, in a fixed order), and
+// the kernel is the undilated one.
+int mdb_conv2d_wgrad_bias_dilated_f32(const float* dy, const float* x, const float* rowscale, float* dw_packed, float* db, int B,
+                                      int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                      int accumulate, void* stream_) {
+    ConvGeom g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation);
+    int rc = check_geom(g);
     if (rc) return rc;
+    if (pad % dilation) return MDB_EUNSUPPORTED;
+    if (!dy || !x || !dw_packed) return MDB_EINVAL;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    if (kh == 1 && stride == 1 && pad == 0) {     // pointwise: one long row of pixels (full 32-pixel reduction tiles)
+        W = B * H * W; H = 1; B = 1;
+        g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation);
+    }
+    const int taps = kh * kw;
+    if (!accumulate) {
+        cudaError_t e = cudaMemsetAsync(dw_packed, 0, sizeof(float) * (size_t)taps * Cout * Cin, stream);
+        if (e != cudaSuccess) return (int)e;
+    }
+    if (db) {
+        rc = mdb_colsum_f32(dy, db, (long long)B * g.Ho * g.Wo, Cout, accumulate, stream_);
+        if (rc) return rc;
+    }
+    const int d = dilation;
+    for (int py = 0; py < d; ++py)
+        for (int px = 0; px < d; ++px) {
+            const int Hc = (g.Ho - py + d - 1) / d, Wc = (g.Wo - px + d - 1) / d;   // the class's dy pixels
+            const int Hx = (H - py + d - 1) / d, Wx = (W - px + d - 1) / d;         // the class's x pixels
+            if (Hc <= 0 || Wc <= 0) continue;
+            rc = wgrad_launch(dy + (size_t)(py * g.Wo + px) * Cout, x + (size_t)(py * W + px) * Cin, rowscale, dw_packed, B, Cin, Cout,
+                              kh, kw, stride, pad / d, Wc, Hc, (uint64_t)d * Cout, (uint64_t)d * g.Wo * Cout,
+                              (uint64_t)g.Ho * g.Wo * Cout, Wx, Hx, (uint64_t)d * Cin, (uint64_t)d * W * Cin, (uint64_t)H * W * Cin,
+                              stream);
+            if (rc) return rc;
+        }
     return 0;
 }
 

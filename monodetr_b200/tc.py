@@ -17,8 +17,8 @@ def _chk(*ts):
             raise RuntimeError("monodetr_b200.tc: contiguous float32 tensors required")
 
 
-def out_size(n, k, s, p):
-    return (n + 2 * p - k) // s + 1
+def out_size(n, k, s, p, d=1):
+    return (n + 2 * p - d * (k - 1) - 1) // s + 1
 
 
 def pack_weight(w_oihw, scale=None):
@@ -190,31 +190,40 @@ def _as_operand(w_packed):
     return split_weights([w_packed], packed_src=True)[0]
 
 
-def conv2d_forward(x, w_packed, bias=None, residual=None, kh=1, kw=1, stride=1, pad=0, relu=False, round_out=False):
-    """w_packed: fp32 (taps, Cout, Cin) or a SplitW (precision mode 'bf16x3')."""
+def conv2d_forward(x, w_packed, bias=None, residual=None, kh=1, kw=1, stride=1, pad=0, relu=False, round_out=False, dilation=1):
+    """w_packed: fp32 (taps, Cout, Cin) or a SplitW (precision mode 'bf16x3').  dilation > 1 (3x3, stride 1) runs the _dilated
+    entry points; dilation 1 the plain ones."""
     w_packed = _as_operand(w_packed)
     split = isinstance(w_packed, SplitW)
     _chk(x, None if split else w_packed, bias, residual)
     B, H, W, Cin = x.shape
     taps, Cout, Cin2 = w_packed.shape
     assert taps == kh * kw and Cin2 == Cin
-    Ho, Wo = out_size(H, kh, stride, pad), out_size(W, kw, stride, pad)
+    Ho, Wo = out_size(H, kh, stride, pad, dilation), out_size(W, kw, stride, pad, dilation)
     y = torch.empty((B, Ho, Wo, Cout), dtype=torch.float32, device=x.device)
     if residual is not None:
         assert residual.shape == y.shape
     flags = int(relu) | (int(round_out) << 1)
-    need = _lib.lib().mdb_conv2d_forward_workspace_bytes(B, H, W, Cin, Cout, kh, kw, stride, pad, flags, int(residual is not None),
-                                                         int(split))
+    if dilation == 1:
+        need = _lib.lib().mdb_conv2d_forward_workspace_bytes(B, H, W, Cin, Cout, kh, kw, stride, pad, flags,
+                                                             int(residual is not None), int(split))
+    else:
+        need = _lib.lib().mdb_conv2d_forward_workspace_bytes_dilated(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags,
+                                                                     int(residual is not None), int(split))
     if need < 0:
         _lib.check(int(need), "conv2d_forward_workspace_bytes")
     if need > 0:
         _ensure_workspace(x.device, need)
-    _lib.call("mdb_conv2d_forward_bf16x3" if split else "mdb_conv2d_forward_f32", x, w_packed.wf if split else w_packed, bias,
-              residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, flags, launches=2 if need > 0 else 1)
+    if dilation == 1:
+        name = "mdb_conv2d_forward_bf16x3" if split else "mdb_conv2d_forward_f32"
+    else:
+        name = "mdb_conv2d_forward_dilated_bf16x3" if split else "mdb_conv2d_forward_dilated_f32"
+    geom = (B, H, W, Cin, Cout, kh, kw, stride, pad) + ((dilation,) if dilation != 1 else ())
+    _lib.call(name, x, w_packed.wf if split else w_packed, bias, residual, y, *geom, flags, launches=2 if need > 0 else 1)
     return y
 
 
-def conv2d_dgrad(dy, w_packed, x_shape, residual=None, relu_mask=None, kh=1, kw=1, stride=1, pad=0, round_out=False):
+def conv2d_dgrad(dy, w_packed, x_shape, residual=None, relu_mask=None, kh=1, kw=1, stride=1, pad=0, round_out=False, dilation=1):
     """w_packed: fp32 (taps, Cout, Cin) or a SplitW with .wd; dy may carry more (zero-padded) channels than a SplitW's O
     as long as both round up to the same number of 32-wide k-blocks."""
     w_packed = _as_operand(w_packed)
@@ -229,12 +238,17 @@ def conv2d_dgrad(dy, w_packed, x_shape, residual=None, relu_mask=None, kh=1, kw=
     else:
         assert dy.shape[-1] == Cout
     dx = torch.empty((B, H, W, Cin), dtype=torch.float32, device=dy.device)
-    _lib.call("mdb_conv2d_dgrad_bf16x3" if split else "mdb_conv2d_dgrad_f32", dy, w_packed.wd if split else w_packed, residual,
-              relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, int(round_out) << 1, launches=stride * stride)
+    if dilation == 1:
+        name = "mdb_conv2d_dgrad_bf16x3" if split else "mdb_conv2d_dgrad_f32"
+    else:
+        name = "mdb_conv2d_dgrad_dilated_bf16x3" if split else "mdb_conv2d_dgrad_dilated_f32"
+    geom = (B, H, W, Cin, Cout, kh, kw, stride, pad) + ((dilation,) if dilation != 1 else ())
+    _lib.call(name, dy, w_packed.wd if split else w_packed, residual, relu_mask, dx, *geom, int(round_out) << 1,
+              launches=stride * stride)
     return dx
 
 
-def conv2d_wgrad(dy, x, rowscale=None, kh=1, kw=1, stride=1, pad=0, with_bias_grad=False):
+def conv2d_wgrad(dy, x, rowscale=None, kh=1, kw=1, stride=1, pad=0, with_bias_grad=False, dilation=1):
     """dw_packed (taps, Cout, Cin); with_bias_grad=True also returns db (Cout,) = dy summed over pixels, produced by the
     same launch (both live in one allocation so a single memset zero-fills them)."""
     _chk(dy, x, rowscale)
@@ -244,8 +258,9 @@ def conv2d_wgrad(dy, x, rowscale=None, kh=1, kw=1, stride=1, pad=0, with_bias_gr
     buf = torch.empty((n + (Cout if with_bias_grad else 0),), dtype=torch.float32, device=x.device)
     dwp = buf[:n].view(kh * kw, Cout, Cin)
     db = buf[n:] if with_bias_grad else None
-    _lib.call("mdb_conv2d_wgrad_bias_f32", dy, x, rowscale, dwp, db, B, H, W, Cin, Cout, kh, kw, stride, pad, 0,
-              launches=1 if (not with_bias_grad or get_precision() != "tf32") else 2)
+    geom = (B, H, W, Cin, Cout, kh, kw, stride, pad) + ((dilation,) if dilation != 1 else ())
+    _lib.call("mdb_conv2d_wgrad_bias_f32" if dilation == 1 else "mdb_conv2d_wgrad_bias_dilated_f32", dy, x, rowscale, dwp, db,
+              *geom, 0, launches=1 if (not with_bias_grad or get_precision() != "tf32") else 2)
     return (dwp, db) if with_bias_grad else dwp
 
 
