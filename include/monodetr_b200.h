@@ -101,6 +101,13 @@ int mdb_msda_fused_forward_f32(const float* value, const int64_t* spatial_shapes
 int mdb_msda_fused_backward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start, const float* offsets,
                                 const float* logits, const float* ref, const float* grad_out, int B, int S, int M, int D, int L, int Lq,
                                 int P, int ref_dim, float* grad_value, float* grad_offsets, float* grad_logits, void* stream);
+/* mdb_msda_fused_backward_f32 for 6-d reference boxes that require a gradient (ref_dim == 6 only): also writes the box partials
+ * ref_part (B,Lq,M,L,4) = [sum d loc_x, sum d loc_y, sum d loc_x off_x, sum d loc_y off_y] over each level's points, reduced in a
+ * fixed order across the unit's lanes.  MDB_EUNSUPPORTED in reproducible mode, like mdb_msda_fused_backward_f32. */
+int mdb_msda_fused_backward_ref_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                    const float* offsets, const float* logits, const float* ref, const float* grad_out, int B, int S,
+                                    int M, int D, int L, int Lq, int P, int ref_dim, float* grad_value, float* grad_offsets,
+                                    float* grad_logits, float* ref_part, void* stream);
 
 /* ---- Tensor-core convolution / linear family (wgmma + TMA, fp32 storage, BF16x3 / TF32 math) ----
  * Replaces the cuDNN / cuBLAS calls behind nn.Conv2d / nn.Linear on the reference path
@@ -271,6 +278,28 @@ int mdb_depth_sample_backward_f32(const float* dout, const float* xy, float* dde
 int mdb_box_refine_forward_f32(const float* tmp, const float* ref, float* y, long long n, int ref_dim, void* stream);
 int mdb_box_refine_backward_f32(const float* dy, const float* y, const float* ref, float* dtmp, float* dref /*or NULL*/, long long n,
                                 int ref_dim, void* stream);
+/* ---- Anchor-box queries (use_dab, dab.cu); every sum runs in a fixed order, no atomics ----------------------------------------
+ * sine embedding (depthaware_transformer.py:29-65, 6-d case): box (n,6) -> out (n,768) = [y | x | l | r | t | b], each block 128
+ * wide: sin of the even, cos of the odd features of (v * 2pi) / dim_t, dim_t[i] = 10000 ** (2 (i // 2) / 128).  backward: dbox (n,6). */
+int mdb_dab_sine_embed_forward_f32(const float* box, float* out, long long n, void* stream);
+int mdb_dab_sine_embed_backward_f32(const float* box, const float* dout, float* dbox, long long n, void* stream);
+/* query position out (B,rows,C) = scale (B,rows,C) * raw, scale NULL = 1; raw (rows,C) shared by all images when `shared`, else
+ * (B,rows,C).  backward: dscale (or NULL) = dqp * raw; draw (or NULL) = dqp * scale, summed over b = 0..B-1 in order when shared. */
+int mdb_dab_query_pos_forward_f32(const float* scale, const float* raw, float* out, int B, long long rows, int C, int shared, void* stream);
+int mdb_dab_query_pos_backward_f32(const float* dqp, const float* scale, const float* raw, float* dscale, float* draw, int B,
+                                   long long rows, int C, int shared, void* stream);
+/* gradient of 6-d reference boxes from the sampling locations of the two-step MSDA path: grad_loc / offsets (B,Lq,M,L,P,2) ->
+ * dref (B,Lq,6), or (Lq,6) summed over the batch when `shared`.  loc = ref_xy + off / P * (l + r, t + b) / 2. */
+int mdb_msda_ref_grad_f32(const float* grad_loc, const float* offsets, int B, int Lq, int M, int L, int P, int shared, float* dref,
+                          void* stream);
+/* the same from the box partials of mdb_msda_fused_backward_ref_f32: ref_part (B,Lq,M,L,4) -> dref (B,Lq,6), or (Lq,6) summed
+ * over the batch when `shared`; 16-byte aligned. */
+int mdb_msda_ref_partials_reduce_f32(const float* ref_part, int B, int Lq, int M, int L, int P, int shared, float* dref, void* stream);
+/* anchors: r, r2 (n) = sigmoid(w) (one copy per consumer), r_batch (B,n) = r repeated over the batch.  backward: dw = (d_sine + d_msda + sum_b d_head[b]) *
+ * r (1 - r); d_sine / d_msda (n) and d_head (B,n) may each be NULL. */
+int mdb_dab_anchor_forward_f32(const float* w, float* r, float* r2, float* r_batch, int B, long long n, void* stream);
+int mdb_dab_anchor_backward_f32(const float* r, const float* d_sine, const float* d_msda, const float* d_head, int B, long long n,
+                                float* dw, void* stream);
 /* depth of a query (monodetr.py:230-262): out[b][q] = ((1/(sigmoid(reg0)+1e-6) - 1) + size3d0 / clamp((c4+c5)*img_h, 1) * fu +
  * grid_sample(weighted_depth, (c01 - 0.5)*2, bilinear, zeros, align_corners=True)) / 3 , reg1.  coord (B,N,6), size3d (B,N,3),
  * depth_reg (B,N,2), wdepth (B,H,W), calibs (B,3,4), img_sizes (B,2) = [W, H].  backward: dwdepth is zero-filled by the call. */

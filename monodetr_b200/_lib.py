@@ -24,6 +24,7 @@ SIGNATURES = {
     "mdb_msda_backward_f64": [_PTR] * 6 + [c_int] * 7 + [_PTR] * 4,
     "mdb_msda_fused_forward_f32": [_PTR] * 6 + [c_int] * 8 + [_PTR, _PTR],
     "mdb_msda_fused_backward_f32": [_PTR] * 7 + [c_int] * 8 + [_PTR] * 4,
+    "mdb_msda_fused_backward_ref_f32": [_PTR] * 7 + [c_int] * 8 + [_PTR] * 5,
     "mdb_msda_prep_forward_f32": [_PTR] * 4 + [c_int] * 6 + [_PTR] * 3,
     "mdb_msda_prep_backward_f32": [_PTR] * 5 + [c_int] * 6 + [_PTR] * 3,
     "mdb_set_deterministic": [c_int],
@@ -65,6 +66,14 @@ SIGNATURES = {
     "mdb_depth_sample_backward_f32": [_PTR] * 3 + [c_int] * 4 + [_PTR],
     "mdb_box_refine_forward_f32": [_PTR] * 3 + [ctypes.c_longlong, c_int, _PTR],
     "mdb_box_refine_backward_f32": [_PTR] * 5 + [ctypes.c_longlong, c_int, _PTR],
+    "mdb_dab_sine_embed_forward_f32": [_PTR] * 2 + [ctypes.c_longlong, _PTR],
+    "mdb_dab_sine_embed_backward_f32": [_PTR] * 3 + [ctypes.c_longlong, _PTR],
+    "mdb_dab_query_pos_forward_f32": [_PTR] * 3 + [c_int, ctypes.c_longlong, c_int, c_int, _PTR],
+    "mdb_dab_query_pos_backward_f32": [_PTR] * 5 + [c_int, ctypes.c_longlong, c_int, c_int, _PTR],
+    "mdb_msda_ref_grad_f32": [_PTR] * 2 + [c_int] * 6 + [_PTR, _PTR],
+    "mdb_msda_ref_partials_reduce_f32": [_PTR] + [c_int] * 6 + [_PTR, _PTR],
+    "mdb_dab_anchor_forward_f32": [_PTR] * 4 + [c_int, ctypes.c_longlong, _PTR],
+    "mdb_dab_anchor_backward_f32": [_PTR] * 4 + [c_int, ctypes.c_longlong, _PTR, _PTR],
     "mdb_head_depth_forward_f32": [_PTR] * 7 + [c_int] * 4 + [_PTR],
     "mdb_head_depth_backward_f32": [_PTR] * 10 + [c_int] * 4 + [_PTR],
     "mdb_depth_tail_forward_f32": [_PTR] * 5 + [ctypes.c_longlong, c_int, c_int, c_int, c_float, _PTR],

@@ -287,15 +287,18 @@ msda_fwd_d32_kernel(const float* __restrict__ value, const int64_t* __restrict__
 // FUSED (LPU == 8 only): `loc` / `attn` are the raw sampling offsets / attention logits, `grad_loc` / `grad_attn` receive the
 // gradients wrt THOSE (the softmax / location pre-processing and its backward, ms_deform_attn.py:145-155, run inside this kernel;
 // the reference points are constants of this path -- the caller takes the unfused path when they need a gradient).
-template <int LPU, int L, bool FUSED = false>
+// REFGRAD (FUSED, 6-d boxes only): also writes, per unit and level, the box partials [sum d loc_x, sum d loc_y,
+// sum d loc_x off_x, sum d loc_y off_y] over the level's points to ref_part (n_units, L, 4), from the lanes' d loc.
+template <int LPU, int L, bool FUSED = false, bool REFGRAD = false>
 __global__ void __launch_bounds__(kThreads, 2)
 msda_bwd_vec_kernel(const float* __restrict__ value, const int64_t* __restrict__ shapes,
                     const int64_t* __restrict__ lsi, const float* __restrict__ loc,
                     const float* __restrict__ attn, const float* __restrict__ grad_out, int S, int M,
                     int Lq, long long n_units, long long units_per_block, float* __restrict__ grad_value,
                     float* __restrict__ grad_loc, float* __restrict__ grad_attn, const float* __restrict__ ref = nullptr,
-                    int ref_dim = 0) {
+                    int ref_dim = 0, float* __restrict__ ref_part = nullptr) {
     static_assert(!FUSED || (LPU == 8 && L == 4), "fused pre-processing: D = 32, L = 4");
+    static_assert(!REFGRAD || FUSED, "box partials: fused path only");
     constexpr int D = 4 * LPU;
     constexpr int UPW = 32 / LPU;
     constexpr int P = 4;
@@ -461,6 +464,23 @@ msda_bwd_vec_kernel(const float* __restrict__ value, const int64_t* __restrict__
                 for (int i = 0; i < 4; ++i) gl[i * 8 + cl] = vals[i] * ((cl & 1) ? sc[i][1] : sc[i][0]);
                 gat[cl] = a0 * (vals[4] - dot);
                 gat[8 + cl] = a1 * (vals[5] - dot);
+            }
+            if constexpr (REFGRAD) {
+                // lane cl holds d loc of (level i, point cl >> 1, component cl & 1), whose raw offset is lp[8 i + cl]: sum over
+                // the level's 4 points = the 4 lanes of equal parity (fixed butterfly), lanes 0 / 1 write x / y
+                float* rp = ref_part + (size_t)unit * (L * 4);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    float s = vals[i], w = vals[i] * __ldg(lp + i * 8 + cl);
+                    s += __shfl_xor_sync(0xffffffffu, s, 2, 8);
+                    w += __shfl_xor_sync(0xffffffffu, w, 2, 8);
+                    s += __shfl_xor_sync(0xffffffffu, s, 4, 8);
+                    w += __shfl_xor_sync(0xffffffffu, w, 4, 8);
+                    if (live && cl < 2) {
+                        rp[i * 4 + cl] = s;
+                        rp[i * 4 + 2 + cl] = w;
+                    }
+                }
             }
         } else if (live) {
             float* gl = grad_loc + (size_t)unit * NLOC;
@@ -798,6 +818,37 @@ int mdb_msda_fused_backward_f32(const float* value, const int64_t* spatial_shape
     const long long upb = ((n_units + grid - 1) / grid + per - 1) / per * per;
     msda_bwd_vec_kernel<8, 4, true><<<grid, kThreads, 0, stream>>>(value, spatial_shapes, level_start, offsets, logits, grad_out, S, M, Lq, n_units,
                                                                    upb, grad_value, grad_offsets, grad_logits, ref, ref_dim);
+    return (int)cudaGetLastError();
+}
+// mdb_msda_fused_backward_f32 for 6-d boxes that require grad, plus the box partials ref_part (B, Lq, M, L, 4) =
+// [sum d loc_x, sum d loc_y, sum d loc_x off_x, sum d loc_y off_y] over each level's points (mdb_msda_ref_partials_reduce_f32
+// turns them into the box gradient).
+int mdb_msda_fused_backward_ref_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                    const float* offsets, const float* logits, const float* ref, const float* grad_out, int B, int S,
+                                    int M, int D, int L, int Lq, int P, int ref_dim, float* grad_value, float* grad_offsets,
+                                    float* grad_logits, float* ref_part, void* stream_) {
+    if (D != 32 || L != 4 || P != 4 || ref_dim != 6) return MDB_EUNSUPPORTED;
+    if (mdb_get_deterministic()) return MDB_EUNSUPPORTED;      // ordered accumulation: mdb_msda_prep_* + mdb_msda_backward_*
+    int rc = check_common(value, spatial_shapes, level_start, offsets, logits, B, S, M, D, L, Lq, P);
+    if (rc) return rc;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const long long n_units = (long long)B * Lq * M;
+    const size_t nv = (size_t)B * S * M * D;
+    if (!aligned16(value) || !aligned16(offsets) || !aligned16(logits) || !aligned16(grad_out) || !aligned16(grad_value))
+        return MDB_EUNSUPPORTED;
+    if (nv) {
+        if (!grad_value) return MDB_EINVAL;
+        cudaError_t e = cudaMemsetAsync(grad_value, 0, sizeof(float) * nv, stream);
+        if (e != cudaSuccess) return (int)e;
+    }
+    if (n_units == 0) return 0;
+    if (!ref || !grad_out || !grad_offsets || !grad_logits || !ref_part) return MDB_EINVAL;
+    const int grid = grid_cap((n_units + 3) / 4, kThreads / 32, num_sms() * 6);
+    const long long per = (kThreads / 32) * 4;
+    const long long upb = ((n_units + grid - 1) / grid + per - 1) / per * per;
+    msda_bwd_vec_kernel<8, 4, true, true><<<grid, kThreads, 0, stream>>>(value, spatial_shapes, level_start, offsets, logits, grad_out, S, M,
+                                                                         Lq, n_units, upb, grad_value, grad_offsets, grad_logits, ref,
+                                                                         ref_dim, ref_part);
     return (int)cudaGetLastError();
 }
 int mdb_msda_backward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start,

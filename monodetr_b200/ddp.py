@@ -3,12 +3,14 @@
 Every gradient-receiving parameter's `.grad` is a view into one contiguous buffer, so backward accumulates
 straight into the bucket and the step ends with a single `all_reduce(bucket) / world_size` over NVLink.  The 15
 tensors that never receive a gradient (sa_v_proj, query_scale, ref_point_head, label_enc -- SURVEY.md appendix C.2)
-are left out of the bucket (their .grad stays None, exactly as in the reference).
+are left out of the bucket (their .grad stays None, exactly as in the reference).  With use_dab, query_scale and
+ref_point_head are on the path and in the bucket; the never-called query_scale_bbox is left out instead.
 """
 import torch
 import torch.distributed as dist
 
 _NEVER_USED = ("sa_v_proj", "decoder.query_scale", "decoder.ref_point_head", "label_enc")
+_NEVER_USED_DAB = ("sa_v_proj", "decoder.query_scale_bbox", "label_enc")
 
 
 class FlatGradBucket:
@@ -25,7 +27,8 @@ class FlatGradBucket:
     ALIGN = 32
 
     def __init__(self, model, views=False):
-        named = [(n, p) for n, p in model.named_parameters() if p.requires_grad and not any(s in n for s in _NEVER_USED)]
+        never = _NEVER_USED_DAB if getattr(model, "use_dab", False) else _NEVER_USED
+        named = [(n, p) for n, p in model.named_parameters() if p.requires_grad and not any(s in n for s in never)]
         # Bucket order = weight-decay tensors first, then the tensors with 'bias' in their name (the reference's optimizer
         # grouping, lib/helpers/optimizer_helper.py:9-16): the fused AdamW (monodetr_b200.optim) then needs one boundary
         # index (`n_decay`, in elements) instead of a per-tensor table.

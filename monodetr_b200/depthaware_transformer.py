@@ -1,7 +1,7 @@
 """Depth-aware transformer -- mirror of lib/models/monodetr/depthaware_transformer.py (DepthAwareTransformer
 :69-312, VisualEncoderLayer/VisualEncoder :315-384, DepthAwareDecoderLayer :387-515, DepthAwareDecoder :518-626,
-build_depthaware_transformer :644-660; default branch only: two_stage / use_dab / two_stage_dino are False in
-configs/monodetr.yaml) with identical parameter names, running on the sm_90a kernels.
+build_depthaware_transformer :644-660; the configs/monodetr.yaml branch and the anchor-box query branch use_dab; two_stage /
+two_stage_dino raise) with identical parameter names, running on the sm_90a kernels.
 
 Tensors are batch-first and token-major ((B, L, C)); feature levels arrive NHWC so flattening is a view.
 """
@@ -186,7 +186,7 @@ class DepthAwareDecoderLayer(nn.Module):
 
 
 class DepthAwareDecoder(nn.Module):
-    def __init__(self, decoder_layer, num_layers, return_intermediate=False, d_model=None):
+    def __init__(self, decoder_layer, num_layers, return_intermediate=False, d_model=None, use_dab=False):
         super().__init__()
         self.layers = _get_clones(decoder_layer, num_layers)
         for i, l in enumerate(self.layers):
@@ -196,14 +196,27 @@ class DepthAwareDecoder(nn.Module):
         self.bbox_embed = None
         self.dim_embed = None
         self.class_embed = None
-        # unused on the default path but part of the reference state_dict (:541-542)
-        self.query_scale = MLP(d_model, d_model, d_model, 2)
-        self.ref_point_head = MLP(d_model, d_model, 2, 2)
+        self.use_dab = use_dab
+        if use_dab:                             # :530-533; query_scale_bbox is never called by the reference
+            self.query_scale = MLP(d_model, d_model, d_model, 2)
+            self.query_scale_bbox = MLP(d_model, 2, 2, 2)
+            self.ref_point_head = MLP(3 * d_model, d_model, d_model, 2)
+        else:
+            # unused on the default path but part of the reference state_dict (:541-542)
+            self.query_scale = MLP(d_model, d_model, d_model, 2)
+            self.ref_point_head = MLP(d_model, d_model, 2, 2)
 
     def forward(self, tgt, reference_points, src, src_spatial_shapes, src_level_start_index, query_pos=None,
                 src_padding_mask=None, depth_pos_embed=None, mask_depth=None, bs=None):
-        """Returns stacked (hs, references (undetached sigmoid boxes), dims) -- see note in MonoDETR.forward."""
+        """Returns stacked (hs, references (undetached sigmoid boxes), dims) -- see note in MonoDETR.forward.
+        use_dab: `reference_points` is Fn.anchors' (sine, msda, head) triple of the anchors and `query_pos` is None; each layer
+        forms its own query position from its boxes (:584-588)."""
         output = tgt
+        raw_pos = None
+        if self.use_dab:
+            # layer 0's boxes are the anchors, the same for every image: sine embedding and ref_point_head on nq rows
+            r_sine, r_msda, reference_points = reference_points
+            raw_pos = self.ref_point_head(Fn.sine_embed(r_sine))
         n_levels = src_spatial_shapes.shape[0]
         intermediate, intermediate_boxes, intermediate_refs, intermediate_dims = [], [], [], []
         # Work that depends on the memory / the depth embedding only is started now on branch streams and joined where each layer
@@ -229,8 +242,18 @@ class DepthAwareDecoder(nn.Module):
         dim_branches = []
         for lid, layer in enumerate(self.layers):
             ahead = {"kv": joined(ahead_kv[lid]), "value": joined(ahead_val[lid])}
+            if self.use_dab:
+                if box_branch is None:
+                    query_pos = Fn.query_pos(None, raw_pos, output.shape[0])           # pos_scale = 1 at layer 0
+                else:
+                    box_branch[0].join(box_branch[1])                              # this layer's position needs its boxes first
+                    raw_pos = self.ref_point_head(Fn.sine_embed(box_branch[1].detach()))
+                    query_pos = Fn.query_pos(self.query_scale(output), raw_pos, output.shape[0])
             if box_branch is None:
-                ref_in = reference_points[:, :, None].expand(-1, -1, n_levels, -1)   # valid_ratios == 1 (:565-571): broadcast over levels
+                if self.use_dab:
+                    ref_in = r_msda                                                 # (nq, 6): shared by the batch and the levels
+                else:
+                    ref_in = reference_points[:, :, None].expand(-1, -1, n_levels, -1)   # valid_ratios == 1 (:565-571): broadcast over levels
             else:
                 ref_in = None
                 ahead["reference_points"] = (lambda bb: lambda: (bb[0].join(bb[1]), bb[1].detach()[:, :, None].expand(-1, -1, n_levels, -1))[1])(box_branch)
@@ -266,8 +289,9 @@ class DepthAwareTransformer(nn.Module):
                  activation="relu", return_intermediate_dec=False, num_feature_levels=4, dec_n_points=4, enc_n_points=4,
                  two_stage=False, two_stage_num_proposals=50, group_num=11, use_dab=False, two_stage_dino=False):
         super().__init__()
-        if two_stage or use_dab or two_stage_dino:
-            raise NotImplementedError("monodetr_b200 implements the configs/monodetr.yaml branch: two_stage / use_dab / two_stage_dino = False")
+        if two_stage or two_stage_dino:
+            raise NotImplementedError("two_stage / two_stage_dino are not implemented: the reference itself fails with them "
+                                      "(two_stage in the training forward, two_stage_dino in every forward)")
         self.d_model, self.nhead, self.group_num = d_model, nhead, group_num
         self.two_stage, self.use_dab, self.two_stage_dino = two_stage, use_dab, two_stage_dino
         self.two_stage_num_proposals = two_stage_num_proposals
@@ -275,9 +299,10 @@ class DepthAwareTransformer(nn.Module):
         self.encoder = VisualEncoder(encoder_layer, num_encoder_layers)
         decoder_layer = DepthAwareDecoderLayer(d_model, dim_feedforward, dropout, activation, num_feature_levels, nhead,
                                                dec_n_points, group_num=group_num)
-        self.decoder = DepthAwareDecoder(decoder_layer, num_decoder_layers, return_intermediate_dec, d_model)
+        self.decoder = DepthAwareDecoder(decoder_layer, num_decoder_layers, return_intermediate_dec, d_model, use_dab=use_dab)
         self.level_embed = nn.Parameter(torch.Tensor(num_feature_levels, d_model))
-        self.reference_points = nn.Linear(d_model, 2)
+        if not use_dab:
+            self.reference_points = nn.Linear(d_model, 2)
         self._reset_parameters()
 
     def _reset_parameters(self):
@@ -287,8 +312,9 @@ class DepthAwareTransformer(nn.Module):
         for m in self.modules():
             if isinstance(m, MSDeformAttn):
                 m._reset_parameters()
-        xavier_uniform_(self.reference_points.weight.data, gain=1.0)
-        constant_(self.reference_points.bias.data, 0.)
+        if not self.use_dab:
+            xavier_uniform_(self.reference_points.weight.data, gain=1.0)
+            constant_(self.reference_points.bias.data, 0.)
         normal_(self.level_embed)
 
     def _shape_tensors(self, shapes, dev):
@@ -303,7 +329,8 @@ class DepthAwareTransformer(nn.Module):
     def forward(self, srcs, masks, pos_embeds, query_embed=None, depth_pos_embed=None, depth_pos_embed_ip=None, attn_mask=None,
                 before_decoder=None):
         """srcs: list of NHWC maps (B, H_l, W_l, C); masks: None (all-False) or list of (B, H_l, W_l) bool;
-        pos_embeds: list of (H_l*W_l, C); query_embed (nq, 2C); depth_pos_embed (B, HW1, C).
+        pos_embeds: list of (H_l*W_l, C); query_embed (nq, 2C), or with use_dab the pair (tgt (nq, C), anchors (nq, 6)) of
+        unactivated embeddings; depth_pos_embed (B, HW1, C).
         Returns hs (L, B, nq, C), init_reference (B, nq, 2), inter_references (L, B, nq, 6), inter_dims (L, B, nq, 3),
         plus the undetached per-layer boxes (list) used by MonoDETR.forward."""
         assert query_embed is not None
@@ -318,11 +345,18 @@ class DepthAwareTransformer(nn.Module):
         spatial_shapes, level_start_index = self._shape_tensors(shapes, dev)
         memory = self.encoder(src_flatten, shapes, spatial_shapes, level_start_index, lvl_pos, mask_flatten)
         c = memory.shape[-1]
-        query_pos, tgt = torch.split(query_embed, c, dim=1)
-        query_pos = query_pos.unsqueeze(0).expand(B, -1, -1)
-        tgt = tgt.unsqueeze(0).expand(B, -1, -1).contiguous()
-        reference_points = Fn.linear(query_pos.contiguous(), self.reference_points.weight, self.reference_points.bias).sigmoid()
-        init_reference_out = reference_points
+        if self.use_dab:                         # :255-260 (the decoder repeats the boxes over the batch, :557-558)
+            tgt, refanchor = query_embed
+            tgt = tgt.unsqueeze(0).expand(B, -1, -1).contiguous()
+            query_pos = None
+            reference_points = Fn.anchors(refanchor, B)
+            init_reference_out = reference_points[2]
+        else:
+            query_pos, tgt = torch.split(query_embed, c, dim=1)
+            query_pos = query_pos.unsqueeze(0).expand(B, -1, -1)
+            tgt = tgt.unsqueeze(0).expand(B, -1, -1).contiguous()
+            reference_points = Fn.linear(query_pos.contiguous(), self.reference_points.weight, self.reference_points.bias).sigmoid()
+            init_reference_out = reference_points
         if before_decoder is not None:           # (the depth predictor may still be running on its own stream: join it here)
             before_decoder()
         hs, inter_references, inter_dims, boxes = self.decoder(tgt, reference_points, memory, spatial_shapes, level_start_index,

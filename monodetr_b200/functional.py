@@ -375,6 +375,175 @@ def msda_prep(off, logits, ref, spatial_shapes, M, L, P):
     return _MsdaPrep.apply(off, logits, ref, spatial_shapes, M, L, P)
 
 
+class _MsdaPrepShared(Function):
+    """_MsdaPrep for 6-d boxes (Lq, 6) shared by every image and level that require grad (the anchors of use_dab's first decoder
+    layer): the box gradient is reduced over (batch, head, level, point) in a fixed order by mdb_msda_ref_grad_f32."""
+
+    @staticmethod
+    def forward(ctx, off, logits, boxes, shapes, M, L, P):
+        B, Lq = off.shape[0], off.shape[1]
+        off = off.contiguous()
+        logits = logits.contiguous()
+        refc = boxes.detach()[None, :, None].expand(B, Lq, L, 6).contiguous()
+        loc = torch.empty((B, Lq, M, L, P, 2), dtype=torch.float32, device=off.device)
+        attn = torch.empty((B, Lq, M, L, P), dtype=torch.float32, device=off.device)
+        _lib.call("mdb_msda_prep_forward_f32", off, logits, refc, shapes, B, Lq, M, L, P, 6, loc, attn)
+        ctx.save_for_backward(attn, refc, shapes, off)
+        ctx.meta = (B, Lq, M, L, P, logits.shape)
+        return loc, attn
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dloc, dattn):
+        attn, refc, shapes, off = ctx.saved_tensors
+        B, Lq, M, L, P, lshape = ctx.meta
+        dloc = dloc.contiguous()
+        dattn = dattn.contiguous()
+        doff = torch.empty_like(off)
+        dlogits = torch.empty(lshape, dtype=torch.float32, device=dloc.device)
+        _lib.call("mdb_msda_prep_backward_f32", dloc, dattn, attn, refc, shapes, B, Lq, M, L, P, 6, doff, dlogits)
+        dboxes = None
+        if ctx.needs_input_grad[2]:
+            dboxes = torch.empty((Lq, 6), dtype=torch.float32, device=dloc.device)
+            _lib.call("mdb_msda_ref_grad_f32", dloc, off, B, Lq, M, L, P, 1, dboxes)
+        return doff, dlogits, dboxes, None, None, None, None
+
+
+class _MsdaFusedSharedBoxes(Function):
+    """_MsdaFused for 6-d boxes (Lq, 6) shared by every image and level that require grad: mdb_msda_fused_backward_ref_f32 also
+    emits per-(image, query, head, level) box partials, which mdb_msda_ref_partials_reduce_f32 sums over the batch, heads and
+    levels in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, value, shapes, lsi, off, logits, boxes):
+        value, off, logits = value.contiguous(), off.contiguous(), logits.contiguous()
+        B, Lq = off.shape[0], off.shape[1]
+        L = shapes.shape[0]
+        refc = boxes.detach()[None, :, None].expand(B, Lq, L, 6).contiguous()
+        out = msda_fused_forward_raw(value, shapes, lsi, off, logits, refc)
+        ctx.save_for_backward(value, shapes, lsi, off, logits, refc)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        value, shapes, lsi, off, logits, refc = ctx.saved_tensors
+        B, S, M, D = value.shape
+        Lq, L = off.shape[1], shapes.shape[0]
+        dout = dout.contiguous()
+        gv, goff, glog = torch.empty_like(value), torch.empty_like(off), torch.empty_like(logits)
+        part = torch.empty((B, Lq, M, L, 4), dtype=torch.float32, device=value.device)
+        _lib.call("mdb_msda_fused_backward_ref_f32", value, shapes, lsi, off, logits, refc, dout, B, S, M, D, L, Lq, 4, 6,
+                  gv, goff, glog, part)
+        dboxes = torch.empty((Lq, 6), dtype=torch.float32, device=value.device)
+        _lib.call("mdb_msda_ref_partials_reduce_f32", part, B, Lq, M, L, 4, 1, dboxes)
+        return gv, None, None, goff, glog, dboxes
+
+
+def msda_shared_boxes(value, spatial_shapes, level_start_index, off, logits, boxes, M, L, P):
+    """MSDA with 6-d reference boxes (Lq, 6) shared by the batch and the levels (value_ratios == 1), differentiable in the boxes.
+    Fused sampling kernels where they apply -- with the box partials when the boxes need a gradient, the plain fused forward
+    when they do not (eval, no_grad) --; reproducible mode takes the two-step path (ordered scatter) with its box reduction."""
+    fused = (value.dtype == torch.float32 and value.shape[-1] == 32 and L == 4 and P == 4 and not os.environ.get("MDB_MSDA_UNFUSED")
+             and not _lib.lib().mdb_get_deterministic())
+    if fused and not (boxes.requires_grad and torch.is_grad_enabled()):
+        B, Lq = off.shape[0], off.shape[1]
+        return msda_fused(value, spatial_shapes, level_start_index, off, logits, boxes.detach()[None, :, None].expand(B, Lq, L, 6))
+    if fused:
+        return _MsdaFusedSharedBoxes.apply(value, spatial_shapes, level_start_index, off, logits, boxes)
+    loc, attn = _MsdaPrepShared.apply(off, logits, boxes, spatial_shapes, M, L, P)
+    return msda(value, spatial_shapes, level_start_index, loc, attn)
+
+
+# ---- anchor-box queries (use_dab; csrc/dab.cu) -----------------------------------------------------------------------
+class _SineEmbed(Function):
+    """gen_sineembed_for_position of 6-d boxes (depthaware_transformer.py:29-65): (..., 6) -> (..., 768)."""
+
+    @staticmethod
+    def forward(ctx, box):
+        boxc = box.detach().contiguous()
+        n = boxc.numel() // 6
+        out = torch.empty((*box.shape[:-1], 768), dtype=torch.float32, device=box.device)
+        _lib.call("mdb_dab_sine_embed_forward_f32", boxc, out, n)
+        ctx.save_for_backward(boxc)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        (boxc,) = ctx.saved_tensors
+        dbox = torch.empty_like(boxc)
+        _lib.call("mdb_dab_sine_embed_backward_f32", boxc, dout.contiguous(), dbox, boxc.numel() // 6)
+        return dbox
+
+
+def sine_embed(box):
+    return _SineEmbed.apply(box)
+
+
+class _QueryPos(Function):
+    """query_pos (B, rows, C) = scale * raw (depthaware_transformer.py:586-588).  scale None: 1; raw (rows, C) shared by the batch
+    (layer 0, whose boxes are the anchors) or (B, rows, C)."""
+
+    @staticmethod
+    def forward(ctx, scale, raw, B):
+        shared = raw.dim() == 2
+        raw = raw.contiguous()
+        scale = None if scale is None else scale.contiguous()
+        rows, C = raw.shape[-2], raw.shape[-1]
+        out = torch.empty((B, rows, C), dtype=torch.float32, device=raw.device)
+        _lib.call("mdb_dab_query_pos_forward_f32", scale, raw, out, B, rows, C, int(shared))
+        ctx.save_for_backward(scale, raw)
+        ctx.meta = (B, rows, C, shared)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dqp):
+        scale, raw = ctx.saved_tensors
+        B, rows, C, shared = ctx.meta
+        dscale = torch.empty_like(scale) if scale is not None and ctx.needs_input_grad[0] else None
+        draw = torch.empty_like(raw) if ctx.needs_input_grad[1] else None
+        _lib.call("mdb_dab_query_pos_backward_f32", dqp.contiguous(), scale, raw, dscale, draw, B, rows, C, int(shared))
+        return dscale, draw, None
+
+
+def query_pos(scale, raw, B):
+    return _QueryPos.apply(scale, raw, B)
+
+
+class _Anchors(Function):
+    """sigmoid(refpoint_embed) (depthaware_transformer.py:256, :557-558) as three outputs, one per consumer, so that the backward
+    adds their gradients in one fixed-order launch: (nq, 6) for the sine embedding, (nq, 6) for the deformable attention and
+    (B, nq, 6) repeated over the batch for the level-0 box.  Separate tensors, not views of one: autograd would otherwise add the
+    consumers' gradients of a shared tensor itself.  The level-0 box copy is materialised because box refinement reads a
+    contiguous (B, nq, 6) reference and returns its gradient in that shape (one row per image, summed here in batch order)."""
+
+    @staticmethod
+    def forward(ctx, w, B):
+        w = w.contiguous()
+        n = w.numel()
+        r, r2 = torch.empty_like(w), torch.empty_like(w)
+        rb = torch.empty((B, *w.shape), dtype=torch.float32, device=w.device)
+        _lib.call("mdb_dab_anchor_forward_f32", w, r, r2, rb, B, n)
+        ctx.save_for_backward(r)
+        ctx.B = B
+        return r, r2, rb
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, d_sine, d_msda, d_head):
+        (r,) = ctx.saved_tensors
+        dw = torch.empty_like(r)
+        c = lambda t: None if t is None else t.contiguous()        # noqa: E731
+        _lib.call("mdb_dab_anchor_backward_f32", r, c(d_sine), c(d_msda), c(d_head), ctx.B, r.numel(), dw)
+        return dw, None
+
+
+def anchors(w, B):
+    return _Anchors.apply(w, B)
+
+
 def msda_fused_forward_raw(value, shapes, lsi, off, logits, refc):
     """mdb_msda_fused_forward_f32 on contiguous tensors (value (B,S,M,32), raw offsets / logits, constant reference points)."""
     B, S, M, D = value.shape

@@ -2,8 +2,9 @@
 with identical constructor arguments, parameter names (state_dict keys incl. the decoder aliases :129-131),
 initialisation rules and forward signature / output dict (:150, :270-283), running on the sm_90a kernels.
 
-Only the configs/monodetr.yaml branch is implemented (with_box_refine=True, two_stage=False, use_dab=False,
-two_stage_dino=False, use_dn=False); other branches raise NotImplementedError instead of silently differing.
+The configs/monodetr.yaml branch (with_box_refine=True, two_stage=False, two_stage_dino=False) is implemented with and without
+the anchor-box queries (use_dab); use_dn changes nothing in the reference model.  two_stage / two_stage_dino / with_box_refine=False
+raise NotImplementedError instead of silently differing.
 """
 import copy
 import math
@@ -38,8 +39,11 @@ class MonoDETR(nn.Module):
                  aux_loss=True, with_box_refine=False, two_stage=False, init_box=False, use_dab=False, group_num=11,
                  two_stage_dino=False):
         super().__init__()
-        if two_stage or use_dab or two_stage_dino or not with_box_refine or num_feature_levels != 4:
-            raise NotImplementedError("monodetr_b200 implements the configs/monodetr.yaml model branch only")
+        if two_stage or two_stage_dino:
+            raise NotImplementedError("two_stage / two_stage_dino are not implemented: the reference itself fails with them "
+                                      "(two_stage in the training forward, two_stage_dino in every forward)")
+        if not with_box_refine or num_feature_levels != 4:
+            raise NotImplementedError("monodetr_b200 implements with_box_refine=True and num_feature_levels=4 only")
         self.num_queries = num_queries
         self.depthaware_transformer = depthaware_transformer
         self.depth_predictor = depth_predictor
@@ -60,7 +64,11 @@ class MonoDETR(nn.Module):
         if init_box:
             nn.init.constant_(self.bbox_embed.layers[-1].weight.data, 0)
             nn.init.constant_(self.bbox_embed.layers[-1].bias.data, 0)
-        self.query_embed = nn.Embedding(num_queries * group_num, hidden_dim * 2)
+        if use_dab:                                 # :74-76
+            self.tgt_embed = nn.Embedding(num_queries * group_num, hidden_dim)
+            self.refpoint_embed = nn.Embedding(num_queries * group_num, 6)
+        else:
+            self.query_embed = nn.Embedding(num_queries * group_num, hidden_dim * 2)
         input_proj_list = []
         for i in range(len(backbone.strides)):
             in_channels = backbone.num_channels[i]
@@ -90,14 +98,18 @@ class MonoDETR(nn.Module):
 
     _NO_PREPACK = ("backbone", "sa_v_proj", "query_scale", "ref_point_head", "sa_qcontent_proj", "sa_qpos_proj",
                    "sa_kcontent_proj", "sa_kpos_proj")
+    # use_dab: query_scale and ref_point_head are GEMMs of every decoder layer; query_scale_bbox is never called
+    _NO_PREPACK_DAB = ("backbone", "sa_v_proj", "query_scale_bbox", "sa_qcontent_proj", "sa_qpos_proj", "sa_kcontent_proj",
+                       "sa_kpos_proj")
 
     def _gemm_weights(self):
         """Every nn.Linear / nn.Conv2d / in_proj slice the forward feeds to the tensor-core GEMMs as-is (the ResNet body
         splits its own BN-folded weights; summed decoder projections are split where they are formed)."""
         out = []
         with torch.no_grad():
+            skip = self._NO_PREPACK_DAB if self.use_dab else self._NO_PREPACK
             for name, m in self.named_modules():
-                if any(k in name for k in self._NO_PREPACK):
+                if any(k in name for k in skip):
                     continue
                 if isinstance(m, nn.MultiheadAttention):
                     w, c = m.in_proj_weight, m.embed_dim
@@ -105,6 +117,14 @@ class MonoDETR(nn.Module):
                 elif isinstance(m, (nn.Linear, nn.Conv2d)):
                     out.append(m.weight)
         return out
+
+    def _query_embeds(self):
+        """The transformer's queries (:182-199): all groups in training, the first num_queries rows in eval.  use_dab: the pair
+        (tgt_embed, refpoint_embed) of weights, which the reference concatenates and the transformer splits again."""
+        if self.use_dab:
+            qe = (self.tgt_embed.weight, self.refpoint_embed.weight)
+            return qe if self.training else tuple(w[:self.num_queries] for w in qe)
+        return self.query_embed.weight if self.training else self.query_embed.weight[:self.num_queries]
 
     def forward(self, images, calibs, targets, img_sizes, dn_args=None):
         """images (B, 3, H, W) fp32 NCHW; calibs (B, 3, 4); targets / dn_args ignored; img_sizes (B, 2) [W, H]."""
@@ -139,7 +159,7 @@ class MonoDETR(nn.Module):
             src = self.input_proj[l](features[-1] if l == len(features) else srcs[-1])
             srcs.append(src)
             pos.append(self.backbone[1](src))
-        query_embeds = self.query_embed.weight if self.training else self.query_embed.weight[:self.num_queries]
+        query_embeds = self._query_embeds()
 
         # The depth predictor and the visual encoder both depend on `srcs` only: the (small) depth branch runs on its own
         # stream beside the encoder and is joined right before the decoder, its first consumer.

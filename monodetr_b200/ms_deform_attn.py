@@ -67,6 +67,13 @@ class MSDeformAttn(nn.Module):
             sampling_offsets, reference_points = sampling_offsets.detach(), reference_points.detach()
         if reference_points.shape[-1] not in (2, 6):
             raise ValueError(f"Last dim of reference_points must be 2 or 6, but get {reference_points.shape[-1]} instead.")
+        if reference_points.dim() == 2:
+            # (Len_q, 6) boxes shared by every image and level (use_dab's anchors at decoder layer 0): differentiable in the boxes
+            if reference_points.shape[-1] != 6:
+                raise ValueError("shared reference boxes must be (Len_q, 6)")
+            output = Fn.msda_shared_boxes(value, input_spatial_shapes, input_level_start_index, sampling_offsets, attention_logits,
+                                          reference_points, self.n_heads, self.n_levels, self.n_points)
+            return Fn.linear(output, self.output_proj.weight, self.output_proj.bias)
         # :145-155 fused: softmax over the 16 (level, point) logits and loc = ref + off / (W_l, H_l)   [2-d refs]
         #                                                     or ref_xy + off / P * (l+r, t+b) / 2    [6-d refs]
         if Fn.msda_fused_applicable(value, reference_points, self.n_levels, self.n_points):

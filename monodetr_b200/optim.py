@@ -9,8 +9,8 @@ bucket's flat gradient buffer as `g`.  `step()` is then a single HBM-bound launc
 parameter) instead of ~10 elementwise kernels per tensor; with `device_step=True` the bias-correction factor is computed
 on the device so the whole step can live inside a CUDA graph.
 
-Parameters that never receive a gradient (SURVEY.md appendix C.2: sa_v_proj, query_scale, ref_point_head, label_enc) are
-not in the bucket and are left untouched, exactly as the reference's `if p.grad is None: continue` (:95-96) leaves them.
+Parameters that never receive a gradient (SURVEY.md appendix C.2: sa_v_proj, query_scale, ref_point_head, label_enc; with
+use_dab sa_v_proj, query_scale_bbox, label_enc) are not in the bucket and are left untouched, exactly as the reference's `if p.grad is None: continue` (:95-96) leaves them.
 """
 import math
 
