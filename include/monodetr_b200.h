@@ -339,6 +339,22 @@ int mdb_adamw_step_f32(float* p, const float* g, float* m, float* v, long long n
                        float one_minus_beta1, float beta2, float one_minus_beta2, float eps, float weight_decay,
                        float step_size, const float* step_size_dev, void* stream);
 
+/* Device-resident schedule of one optimizer: what a captured CUDA graph reads every replay instead of host floats.  The caller
+ * owns the block (40 bytes, 8-byte aligned, device memory), initialises t (the number of steps taken so far, an integer value)
+ * and the three hyper-parameters as the DOUBLES the host holds, and may overwrite lr between steps with an asynchronous copy
+ * ordered on the training stream (a learning-rate schedule then reaches a graph that was captured earlier). */
+typedef struct MdbAdamwHyper {
+    double t;         /* steps taken; mdb_adamw_advance adds 1 */
+    double lr;
+    double beta1;
+    double beta2;
+    float step_size;  /* written by mdb_adamw_advance; pass its address as mdb_adamw_step_f32's step_size_dev */
+    float reserved_;
+} MdbAdamwHyper;
+/* One single-thread launch: t += 1; step_size = (float)(lr * sqrt(1 - beta2^t) / (1 - beta1^t)), every operation in fp64 in
+ * that order and one rounding to fp32 -- the value optimizer_helper.py:122-124 computes on the host. */
+int mdb_adamw_advance(MdbAdamwHyper* hyper, void* stream);
+
 /* ---- Inference post-process on the device (decode.cu) -- SURVEY.md 8 f3 ----
  * extract: lib/helpers/decode_helper.py:57-110 (extract_dets_from_outputs).  logits (B,Q,C), boxes (B,Q,6) cx cy l r t b,
  * dim3 (B,Q,3), depth (B,Q,2) [depth, log-variance], angle (B,Q,24).  dets (B,topk,37) = label, score, xs2d, ys2d, w, h, depth,
@@ -407,6 +423,14 @@ int mdb_criterion_losses_backward_f32(int L, const float* const* logits, const f
                                       int group, int Gmax, float focal_alpha, float world_size, const float* grad_losses,
                                       const float* aux, float* const* dlogits, float* const* dboxes, float* const* ddim3, float* const* ddepth,
                                       float* const* dangle, void* stream);
+
+/* ---- Loss log of the training loop (trainlog.cu) -- lib/helpers/trainer_helper.py:145-152 without the 26 `.item()` calls ----
+ * Appends one record to a device ring: record k = *counter % slots receives values[i] * weights[i] (one fp32 multiply each, the
+ * bits of `(loss * weight).item()`) for i < n, then their sum in index order at position n; afterwards *counter += 1.  The slot
+ * index comes from device memory, so a captured launch is the same every replay; the host, which counts its own pushes, knows
+ * which record a step went to and copies it out when it wants to print.  ring: slots * (n + 1) floats; counter: one int64 the
+ * caller zeroes; 1 <= n <= 255, slots >= 1. */
+int mdb_trainlog_push_f32(const float* values, const float* weights, int n, float* ring, int slots, long long* counter, void* stream);
 
 /* ---- Input pipeline on the device (preprocess.cu) -- SURVEY.md 8 f4 ----
  * lib/datasets/kitti/kitti_dataset.py:140-161: [flip] -> PIL Image.transform(AFFINE, BILINEAR) -> float32 / 255 -> (x - mean) / std -> CHW.

@@ -262,6 +262,73 @@ def weighted_sum(crit):
     return (losses * _weight_matrix(crit, losses.shape[0], losses.device)).sum()
 
 
+class LossLog:
+    """The trainer's loss log (lib/helpers/trainer_helper.py:145-152) without a host synchronisation per step.  `push()` -- one
+    launch, graph-safe -- appends the weighted loss table of the criterion's last forward to a device ring; `fetch(step)` starts
+    an asynchronous copy of that step's record into pinned memory and returns a handle whose `ready()` polls an event behind
+    the copy and whose `read()` gives the reference's log dict: every term of `weight_dict` as `(loss * weight).item()` would
+    return it, in the criterion's dict order, and `loss_detr` = their sum accumulated in Python floats in that order."""
+
+    def __init__(self, crit, n_layers, device, slots=64):
+        self.crit, self.L, self.slots, self.n = crit, n_layers, slots, n_layers * NUM_LOSSES
+        self.ring = torch.zeros(slots, self.n + 1, dtype=torch.float32, device=device)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=device)
+        self.pushed = 0                                                       # host mirror of the device counter
+        want = [k for l in crit.losses for k in _GROUPS[l]]
+        self.terms = []                                                       # (name, index into the flattened table)
+        for li in range(n_layers):
+            for k in want:
+                name = _NAMES[k] + ("" if li == 0 else f"_{li - 1}")
+                if not (li > 0 and k in (DEPTH_MAP, CLASS_ERROR)) and name in crit.weight_dict:
+                    self.terms.append((name, li * NUM_LOSSES + k))
+
+    def push(self):
+        losses = self.crit._last_losses
+        _lib.call("mdb_trainlog_push_f32", losses, _weight_matrix(self.crit, self.L, losses.device), self.n, self.ring, self.slots,
+                  self.counter)
+        if not (torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()):
+            self.pushed += 1                                                  # a captured push runs at replay: see replayed()
+
+    def replayed(self):
+        """Tell the host mirror that a graph holding a captured `push()` has been replayed once."""
+        self.pushed += 1
+
+    def fetch(self, step):
+        """`step`: 0 for the first push ever, 1 for the second, ...; at most `slots` pushes may have followed it."""
+        if not 0 <= self.pushed - 1 - step < self.slots:
+            raise ValueError("LossLog.fetch: that step is no longer in the ring")
+        rec = self.ring[step % self.slots]
+        world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        if world > 1:                                                          # misc.reduce_dict: the mean over ranks
+            rec = rec.clone()
+            dist.all_reduce(rec)
+            rec /= world
+        host = torch.empty(self.n + 1, dtype=torch.float32, pin_memory=rec.device.type == "cuda")
+        host.copy_(rec, non_blocking=True)
+        event = torch.cuda.Event() if rec.device.type == "cuda" else None
+        if event is not None:
+            event.record()
+        return _LogRecord(host, event, sorted(self.terms) if world > 1 else self.terms)
+
+
+class _LogRecord:
+    def __init__(self, host, event, terms):
+        self.host, self.event, self.terms = host, event, terms
+
+    def ready(self):
+        return self.event is None or self.event.query()
+
+    def read(self):
+        if self.event is not None and not self.event.query():
+            self.event.synchronize()
+        values, log, total = self.host.tolist(), {}, 0
+        for name, i in self.terms:
+            log[name] = values[i]
+            total += log[name]
+        log["loss_detr"] = total
+        return log
+
+
 def build_weight_dict(cfg):
     """monodetr.py:578-601 (without the dn terms, which need use_dn -- SURVEY.md: not on the path)."""
     w = {"loss_ce": cfg["cls_loss_coef"], "loss_bbox": cfg["bbox_loss_coef"], "loss_giou": cfg["giou_loss_coef"],

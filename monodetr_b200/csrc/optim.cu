@@ -53,7 +53,23 @@ adamw_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __r
         adamw1(p[e], g[e], m[e], v[e], b1, omb1, b2, omb2, eps, e < n_decay ? wd : 0.f, neg_step);
 }
 
+// One thread: t += 1 and the bias-corrected step size of that t.  Every operation is a separately rounded fp64 operation in
+// the order of the host expression lr * sqrt(1 - beta2 ** t) / (1 - beta1 ** t); the result is rounded to fp32 once.
+__global__ void adamw_advance_kernel(MdbAdamwHyper* h) {
+    const double t = h->t + 1.0;
+    const double bc2 = __dsub_rn(1.0, pow(h->beta2, t));
+    const double bc1 = __dsub_rn(1.0, pow(h->beta1, t));
+    h->t = t;
+    h->step_size = (float)__ddiv_rn(__dmul_rn(h->lr, sqrt(bc2)), bc1);
+}
+
 }  // namespace
+
+extern "C" int mdb_adamw_advance(MdbAdamwHyper* hyper, void* stream) {
+    if (!hyper || (reinterpret_cast<uintptr_t>(hyper) & 7u)) return MDB_EINVAL;
+    adamw_advance_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream)>>>(hyper);
+    return (int)cudaGetLastError();
+}
 
 extern "C" int mdb_adamw_step_f32(float* p, const float* g, float* m, float* v, long long n, long long n_decay, float beta1,
                                   float one_minus_beta1, float beta2, float one_minus_beta2, float eps, float weight_decay,
