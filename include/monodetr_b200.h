@@ -300,6 +300,15 @@ int mdb_msda_ref_partials_reduce_f32(const float* ref_part, int B, int Lq, int M
 int mdb_dab_anchor_forward_f32(const float* w, float* r, float* r2, float* r_batch, int B, long long n, void* stream);
 int mdb_dab_anchor_backward_f32(const float* r, const float* d_sine, const float* d_msda, const float* d_head, int B, long long n,
                                 float* dw, void* stream);
+/* ---- Learned position embedding (position_embedding: 'learned' / 'v3', pos_embed.cu); no atomics, nothing allocated ----------
+ * col, row (50,128) tables.  For a map of H x W: i = x / W * 49 (fp32, each operation rounded), f = floor(i), c = min(f + 1, 49),
+ * d = i - f; x_emb[x] = col[f] (1 - d) + col[c] d, y_emb[y] likewise from row over H.  out (H*W,256) channels-last:
+ * out[y*W + x] = [x_emb[x] | y_emb[y]] (column embedding first), bit-identical to the separately rounded fp32 operations;
+ * col, row and out 16-byte aligned.  backward: dpos (H*W,256) (summed over the batch) -> dcol, drow (50,128); every row is written
+ * (zero where no coordinate reaches it), summed per row over the coordinates in ascending order, each the ascending sum over the
+ * other axis times (1 - d) or d. */
+int mdb_pos_learned_forward_f32(const float* col, const float* row, int H, int W, float* out, void* stream);
+int mdb_pos_learned_backward_f32(const float* dpos, int H, int W, float* dcol, float* drow, void* stream);
 /* depth of a query (monodetr.py:230-262): out[b][q] = ((1/(sigmoid(reg0)+1e-6) - 1) + size3d0 / clamp((c4+c5)*img_h, 1) * fu +
  * grid_sample(weighted_depth, (c01 - 0.5)*2, bilinear, zeros, align_corners=True)) / 3 , reg1.  coord (B,N,6), size3d (B,N,3),
  * depth_reg (B,N,2), wdepth (B,H,W), calibs (B,3,4), img_sizes (B,2) = [W, H].  backward: dwdepth is zero-filled by the call. */

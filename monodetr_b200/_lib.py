@@ -74,6 +74,8 @@ SIGNATURES = {
     "mdb_msda_ref_partials_reduce_f32": [_PTR] + [c_int] * 6 + [_PTR, _PTR],
     "mdb_dab_anchor_forward_f32": [_PTR] * 4 + [c_int, ctypes.c_longlong, _PTR],
     "mdb_dab_anchor_backward_f32": [_PTR] * 4 + [c_int, ctypes.c_longlong, _PTR, _PTR],
+    "mdb_pos_learned_forward_f32": [_PTR] * 2 + [c_int] * 2 + [_PTR, _PTR],
+    "mdb_pos_learned_backward_f32": [_PTR] + [c_int] * 2 + [_PTR] * 3,
     "mdb_head_depth_forward_f32": [_PTR] * 7 + [c_int] * 4 + [_PTR],
     "mdb_head_depth_backward_f32": [_PTR] * 10 + [c_int] * 4 + [_PTR],
     "mdb_depth_tail_forward_f32": [_PTR] * 5 + [ctypes.c_longlong, c_int, c_int, c_int, c_float, _PTR],

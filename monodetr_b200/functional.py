@@ -544,6 +544,33 @@ def anchors(w, B):
     return _Anchors.apply(w, B)
 
 
+# ---- learned position embedding (position_embedding: 'learned'; csrc/pos_embed.cu) --------------------------------------
+class _PosLearned(Function):
+    """PositionEmbeddingLearned.forward (position_encoding.py:68-86) for an H x W map: the (H*W, 256) table [col | row] of the two
+    interpolated (50, 128) tables.  It depends on the map's size only, so nothing is saved; the backward takes the table's
+    gradient, which autograd has already summed over its consumers, and returns both tables' gradients in one launch."""
+
+    @staticmethod
+    def forward(ctx, col, row, H, W):
+        out = torch.empty((H * W, 2 * col.shape[1]), dtype=torch.float32, device=col.device)
+        _lib.call("mdb_pos_learned_forward_f32", col.detach().contiguous(), row.detach().contiguous(), H, W, out)
+        ctx.hw = (H, W)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dpos):
+        H, W = ctx.hw
+        dcol = torch.empty((50, 128), dtype=torch.float32, device=dpos.device)
+        drow = torch.empty_like(dcol)
+        _lib.call("mdb_pos_learned_backward_f32", dpos.contiguous(), H, W, dcol, drow)
+        return dcol, drow, None, None
+
+
+def pos_learned(col, row, H, W):
+    return _PosLearned.apply(col, row, H, W)
+
+
 def msda_fused_forward_raw(value, shapes, lsi, off, logits, refc):
     """mdb_msda_fused_forward_f32 on contiguous tensors (value (B,S,M,32), raw offsets / logits, constant reference points)."""
     B, S, M, D = value.shape

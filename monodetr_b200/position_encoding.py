@@ -1,12 +1,17 @@
-"""Sine position embedding -- mirror of lib/models/monodetr/position_encoding.py:20-56 (PositionEmbeddingSine,
-normalize=True, 128+128 features, temperature 10000) for the all-False masks this path always has
-(backbone.py:88, monodetr.py:173-174): y_embed = (row+1)/(H+1e-6)*2pi, x_embed likewise.  Input-independent, so
-it is computed once per (H, W, device) and cached; layout is token-major (H*W, 256) to match NHWC activations.
+"""Position embeddings -- mirror of lib/models/monodetr/position_encoding.py for the all-False masks this path always has
+(backbone.py:88, monodetr.py:173-174); layout is token-major (H*W, 256) to match NHWC activations.
+
+  * PositionEmbeddingSine (:20-56, normalize=True, 128+128 features, temperature 10000): y_embed = (row+1)/(H+1e-6)*2pi, x_embed
+    likewise, channels [pos_y | pos_x].  Input-independent, so it is computed once per (H, W, device) and cached.
+  * PositionEmbeddingLearned (:59-86): two (50, 128) tables interpolated at x / W * 49 and y / H * 49, channels [col (x) | row (y)]
+    -- the opposite order of the sine table.  Its tables train, so it is recomputed every call (one launch, csrc/pos_embed.cu).
 """
 import math
 
 import torch
 from torch import nn
+
+from . import functional as Fn
 
 
 class PositionEmbeddingSine(nn.Module):
@@ -44,8 +49,29 @@ class PositionEmbeddingSine(nn.Module):
         return self.table(H, W, feat_nhwc.device)
 
 
+class PositionEmbeddingLearned(nn.Module):
+    """Same parameters (row_embed, col_embed: nn.Embedding(50, num_pos_feats), N(0, 1)) as the reference.  The kernels hold 128
+    features per table (hidden_dim 256, which the depth predictor assumes as well)."""
+
+    def __init__(self, num_pos_feats=256):
+        super().__init__()
+        if num_pos_feats != 128:
+            raise NotImplementedError(f"monodetr_b200 position_embedding 'learned' implements hidden_dim 256 (num_pos_feats 128), "
+                                      f"not num_pos_feats {num_pos_feats}")
+        self.row_embed = nn.Embedding(50, num_pos_feats)
+        self.col_embed = nn.Embedding(50, num_pos_feats)
+
+    def forward(self, feat_nhwc):
+        """feat (B, H, W, C) -> (H*W, 2*num_pos_feats) = [x_emb | y_emb], identical for every image of the batch."""
+        _, H, W, _ = feat_nhwc.shape
+        return Fn.pos_learned(self.col_embed.weight, self.row_embed.weight, H, W)
+
+
 def build_position_encoding(cfg):
     n_steps = cfg["hidden_dim"] // 2
     if cfg["position_embedding"] in ("v2", "sine"):
         return PositionEmbeddingSine(n_steps, normalize=True)
-    raise NotImplementedError("monodetr_b200 implements position_embedding: 'sine' (configs/monodetr.yaml)")
+    if cfg["position_embedding"] in ("v3", "learned"):
+        return PositionEmbeddingLearned(n_steps)
+    raise NotImplementedError("monodetr_b200 implements position_embedding: 'sine' / 'v2' and 'learned' / 'v3' "
+                              "(configs/monodetr.yaml)")
