@@ -177,9 +177,25 @@ add_ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, con
 
 // ---------------------------------------------------------------------------------------------------
 // GroupNorm on NHWC: x[B][HW][C], G groups of C/G = 8 channels.
-// stats[b][g] = {sum, sumsq} in double (atomics), then a normalise pass.
+// stats[b][g] = {sum, sumsq} of the SHIFTED values x - K[b][g], then a normalise pass.  A thread adds each pixel's float4 in
+// fp32 and accumulates in double (a long fp32 chain lost ~1e-5 of a group's variance when one thread owned a whole group).
+// K[b][g] = x[b][pixel 0][first channel of g] (gn_shift): every thread that sums a group subtracts the same K, so the sums
+// see values of the group's spread rather than of its offset, and sumsq / n - (sum / n)^2 does not cancel the offset's
+// digits away (raw sums lose ~mean^2 / var of the variance's precision; a constant group is exactly 0, so y = beta).
 // ---------------------------------------------------------------------------------------------------
 constexpr int GN_THREADS = 256;
+
+__device__ __forceinline__ float gn_shift(const float* __restrict__ x, int b, int g, int HW, int C, int G) {
+    return x[(size_t)b * HW * C + g * (C / G)];
+}
+
+// mean and rstd of group (b, g) from its shifted sums: var clamped at 0 (as PyTorch does) before eps
+__device__ __forceinline__ void gn_mean_rstd(const double* __restrict__ stats, float K, int b, int g, int G, double inv_n,
+                                             float eps, float& mean, float& rstd) {
+    const double d = stats[((size_t)b * G + g) * 2] * inv_n, sq = stats[((size_t)b * G + g) * 2 + 1] * inv_n;
+    mean = (float)((double)K + d);
+    rstd = rsqrtf((float)fmax(sq - d * d, 0.0) + eps);
+}
 
 // thread t: channel quad cq = t % (C/4), pixel lane pl = t / (C/4); C/4 must divide 256 (C in {64,128,256,512,1024})
 __global__ void __launch_bounds__(GN_THREADS)
@@ -188,15 +204,17 @@ gn_stats_kernel(const float* __restrict__ x, double* __restrict__ stats, int HW,
     const int cq_n = C / 4;
     const int cq = threadIdx.x % cq_n, pl = threadIdx.x / cq_n, pls = GN_THREADS / cq_n;
     const int p0 = blockIdx.x * pix_per_block, p1 = min(HW, p0 + pix_per_block);
-    float s = 0.f, ss = 0.f;
+    const float K = gn_shift(x, b, cq * 4 / (C / G), HW, C, G);
+    double s = 0.0, ss = 0.0;
     for (int p = p0 + pl; p < p1; p += pls) {
-        const float4 v = *reinterpret_cast<const float4*>(x + ((size_t)b * HW + p) * C + cq * 4);
+        float4 v = *reinterpret_cast<const float4*>(x + ((size_t)b * HW + p) * C + cq * 4);
+        v.x -= K; v.y -= K; v.z -= K; v.w -= K;
         s += v.x + v.y + v.z + v.w;
         ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
     }
     // channels per group = C/G; quads per group = C/G/4 (2 for 8-channel groups)
     const int qpg = C / G / 4;
-    __shared__ float sh[2][GN_THREADS];
+    __shared__ double sh[2][GN_THREADS];
     sh[0][threadIdx.x] = s;
     sh[1][threadIdx.x] = ss;
     __syncthreads();
@@ -226,10 +244,8 @@ gn_apply_kernel(const float* __restrict__ x, const double* __restrict__ stats, c
         const int c = (int)(e % C);
         const int b = (int)(e / ((long long)HW * C));
         const int g = c / cpg;
-        const double su = stats[((size_t)b * G + g) * 2], sq = stats[((size_t)b * G + g) * 2 + 1];
-        const double mu = su * inv_n;
-        const float mean = (float)mu;
-        const float rstd = rsqrtf((float)(sq * inv_n - mu * mu) + eps);
+        float mean, rstd;
+        gn_mean_rstd(stats, gn_shift(x, b, g, HW, C, G), b, g, G, inv_n, eps, mean, rstd);
         const float4 v = *reinterpret_cast<const float4*>(x + e);
         const float4 ga = *reinterpret_cast<const float4*>(gamma + c);
         const float4 be = *reinterpret_cast<const float4*>(beta + c);
@@ -433,9 +449,11 @@ gn_stats_group_kernel(const float* __restrict__ x, double* __restrict__ stats, i
     const int g = blockIdx.x, b = blockIdx.y;
     const int qpg = C / G / 4, q = threadIdx.x % qpg, pl = threadIdx.x / qpg, pls = GN_THREADS / qpg;
     const float* xp = x + (size_t)b * HW * C + g * (C / G) + q * 4;
-    float s = 0.f, ss = 0.f;
+    const float K = gn_shift(x, b, g, HW, C, G);
+    double s = 0.0, ss = 0.0;
     for (int p = pl; p < HW; p += pls) {
-        const float4 v = *reinterpret_cast<const float4*>(xp + (size_t)p * C);
+        float4 v = *reinterpret_cast<const float4*>(xp + (size_t)p * C);
+        v.x -= K; v.y -= K; v.z -= K; v.w -= K;
         s += v.x + v.y + v.z + v.w;
         ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
     }

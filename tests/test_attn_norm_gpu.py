@@ -81,7 +81,8 @@ def test_attention_dropout_statistics_and_determinism():
     assert float((dv_bad - dv).abs().max()) > 1e-3
 
 
-@pytest.mark.parametrize("M,C,with_res", [(1000, 256, True), (81600, 256, True), (333, 256, False), (77, 512, True), (64, 128, True)])
+@pytest.mark.parametrize("M,C,with_res", [(1000, 256, True), (81600, 256, True), (333, 256, False), (77, 512, True), (64, 128, True),
+                                          (1, 128, True), (7, 512, False)])
 def test_add_layernorm(M, C, with_res):
     from monodetr_b200 import kernels as K
     g = torch.Generator(device="cuda").manual_seed(M)
@@ -117,7 +118,8 @@ def test_add_layernorm_dropout():
     assert 0.88 < float(keep.float().mean()) < 0.92
 
 
-@pytest.mark.parametrize("B,HW,C,relu", [(2, 1920, 256, False), (2, 1920, 256, True), (3, 7680, 256, False), (2, 120, 256, True), (1, 77, 64, False)])
+@pytest.mark.parametrize("B,HW,C,relu", [(2, 1920, 256, False), (2, 1920, 256, True), (3, 7680, 256, False), (2, 120, 256, True), (1, 77, 64, False),
+                                         (9, 257, 512, True), (2, 1, 1024, False)])
 def test_groupnorm(B, HW, C, relu):
     from monodetr_b200 import kernels as K
     G = 32 if C >= 256 else 8

@@ -41,7 +41,7 @@ def _twice(fn):
 
 
 # ---- LayerNorm -------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("M,C", [(1000, 128), (81600, 256), (4400, 256), (777, 512)])
+@pytest.mark.parametrize("M,C", [(1000, 128), (81600, 256), (4400, 256), (777, 512), (3, 256)])
 def test_layernorm_backward(repro, M, C):
     g = torch.Generator(device="cuda").manual_seed(M + C)
     x, r, dy = (torch.randn(M, C, device="cuda", generator=g) for _ in range(3))
@@ -63,6 +63,8 @@ def test_layernorm_backward(repro, M, C):
         assert torch.equal(a, b)                                  # same per-row kernels in both modes
     assert _rel(dg, dflt[3]) < 1e-5 and _rel(db, dflt[4]) < 1e-5
     assert torch.allclose(ag, prior_g + dg, rtol=1e-6, atol=1e-6) and torch.allclose(ab, prior_b + db, rtol=1e-6, atol=1e-6)
+    # accumulate = 1 in the default mode: atomics onto the prior, in another order than the accumulate = 0 call's
+    assert _rel(dflt[5], prior_g + dflt[3]) < 1e-5 and _rel(dflt[6], prior_b + dflt[4]) < 1e-5
     # against torch without dropout (the mask of the kernels is a hash, not torch's RNG)
     yn, mean, rstd = K.add_layernorm_forward(x, r, gamma, beta, 1e-5)
     _, _, dgn, dbn = K.add_layernorm_backward(dy, x, r, gamma, mean, rstd)
