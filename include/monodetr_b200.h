@@ -568,6 +568,15 @@ int mdb_kitti_eval(const int* gt_off, const int* dt_off, const long long* ov_off
                    int max_dt, long long n_ov, const double* gt_f, const int* gt_i, const double* dt_f, const int* dt_cls,
                    const double* overlaps, const int* classes, const double* min_overlaps, int n_cls, int compute_aos,
                    void* workspace, long long workspace_bytes, double* result, void* stream);
+/* The distance-binned evaluation (eval.py:85-159 clean_data_by_distance, DISTANCE_COVER = False, as do_eval(..., DIForDIS=False)
+ * runs it): mdb_kitti_eval with the third configuration index a distance bin instead of a difficulty, cfg = ((metric * n_cls + m)
+ * * 3 + bin) * 2 + k.  Bin 0 keeps the gt with ||location|| <= 30 m, bin 1 those in (30, 50] m, bin 2 those in (50, 70] m
+ * (fp64 x*x + y*y + z*z in that order, correctly rounded square root); the others are ignored.  Every bin applies the hard level's
+ * occlusion / truncation / height limits to gt and its height limit (25) to detections.  Same arguments, workspace and launches. */
+int mdb_kitti_eval_distance(const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int n_gt, int n_dt,
+                            int max_gt, int max_dt, long long n_ov, const double* gt_f, const int* gt_i, const double* dt_f,
+                            const int* dt_cls, const double* overlaps, const int* classes, const double* min_overlaps, int n_cls,
+                            int compute_aos, void* workspace, long long workspace_bytes, double* result, void* stream);
 
 /* Detections of a validation pass kept on the device instead of result files (tester_helper.py:112-132 writes them,
  * kitti_common.py:294-347 reads them back).  mdb_kitti_collect_dets_f32 takes mdb_decode_dets_f32's rows (B, topk, 14) and

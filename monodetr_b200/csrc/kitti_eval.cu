@@ -3,7 +3,7 @@
 // loops and one JIT-compiled CUDA kernel.  Inputs are packed on the host in CSR form (per-image offsets into flat gt / detection
 // tables, include/monodetr_b200.h).  Six kernels in two entry points, no host synchronisation, no device allocation:
 //   * overlaps    eval.py:162-230, rotate_iou.py:17-330   one CTA per image: the dt x gt block of the image, 3 metrics
-//   * clean       eval.py:30-82                           one CTA per (class, difficulty): ignored flags, valid-gt count
+//   * clean       eval.py:30-82 (85-159 by distance)      one CTA per (class, difficulty or bin): ignored flags, valid-gt count
 //   * pass 1      eval.py:233-350 (compute_fp=False)      one warp per (configuration, image): the matched TP scores
 //   * thresholds  eval.py:9-27                            one CTA per configuration: bitonic sort, then the 41-point ranks
 //   * pass 2      eval.py:365-412 (compute_fp=True)       one warp per (configuration, image, threshold): tp / fp / fn / AOS
@@ -184,21 +184,31 @@ __global__ void __launch_bounds__(128) overlaps_kernel(const int* __restrict__ g
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // clean_data (eval.py:30-82) for one (class m, difficulty l) per CTA: ignored_gt / ignored_dt in {-1, 0, 1} and num_valid_gt.
+// BY_DISTANCE: clean_data_by_distance (eval.py:85-159, DISTANCE_COVER = False) for one (class m, distance bin l) per CTA.  Every
+// bin takes the hard level's limits, and a gt is also ignored outside its bin of ||location||: (0, 30], (30, 50], (50, 70] m
+// (the first bin has no lower edge).  The norm is fp64 x*x + y*y + z*z, left to right and correctly rounded.
+template <bool BY_DISTANCE>
 __global__ void __launch_bounds__(256) clean_kernel(const double* __restrict__ gt_f, const int* __restrict__ gt_i,
                                                     const double* __restrict__ dt_f, const int* __restrict__ dt_cls,
                                                     const int* __restrict__ classes, int n_gt, int n_dt, signed char* __restrict__ ign_gt,
                                                     signed char* __restrict__ ign_dt, int* __restrict__ n_valid) {
     const int ml = blockIdx.x, m = ml / 3, l = ml - m * 3;
     const int cls = classes[m];
-    const double min_height = l == 0 ? 40.0 : 25.0, max_trunc = l == 0 ? 0.15 : (l == 1 ? 0.3 : 0.5);   // eval.py:32-34
-    const int max_occ = l;
+    const int lv = BY_DISTANCE ? 2 : l;                                                   // the level whose limits apply
+    const double min_height = lv == 0 ? 40.0 : 25.0, max_trunc = lv == 0 ? 0.15 : (lv == 1 ? 0.3 : 0.5);   // eval.py:32-34
+    const int max_occ = lv;
     int mine = 0;
     for (int g = threadIdx.x; g < n_gt; g += blockDim.x) {
         const double* f = gt_f + (size_t)g * kGtCols;
         const int occ = gt_i[g * 3 + 0], code = gt_i[g * 3 + 1];
         const int valid = code == cls ? 1 : ((cls == 1 && code == 4) || (cls == 0 && code == 3)) ? 0 : -1;
         const double height = __dsub_rn(f[3], f[1]);
-        const bool ignore = occ > max_occ || f[5] > max_trunc || height <= min_height;
+        bool ignore = occ > max_occ || f[5] > max_trunc || height <= min_height;
+        if (BY_DISTANCE) {                                                                // eval.py:112, 121-133
+            const double dis = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(f[6], f[6]), __dmul_rn(f[7], f[7])), __dmul_rn(f[8], f[8])));
+            const double hi = l == 0 ? 30.0 : (l == 1 ? 50.0 : 70.0), lo = l == 1 ? 30.0 : 50.0;
+            ignore = ignore || dis > hi || (l > 0 && dis <= lo);
+        }
         signed char v;
         if (valid == 1 && !ignore) { v = 0; ++mine; }
         else if (valid == 0 || (ignore && valid == 1)) v = 1;
@@ -602,10 +612,13 @@ extern "C" long long mdb_kitti_eval_workspace_bytes(int n_img, int n_gt, int n_d
     return (long long)layout(n_img, n_gt, n_dt, n_cls, compute_aos).total;
 }
 
-extern "C" int mdb_kitti_eval(const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int n_gt, int n_dt,
-                              int max_gt, int max_dt, long long n_ov, const double* gt_f, const int* gt_i, const double* dt_f,
-                              const int* dt_cls, const double* overlaps, const int* classes, const double* min_overlaps, int n_cls,
-                              int compute_aos, void* workspace, long long workspace_bytes, double* result, void* stream) {
+namespace {
+
+// Both entry points: the configurations differ only in how clean_kernel assigns the third index (difficulty or distance bin).
+int kitti_eval_impl(bool by_distance, const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int n_gt, int n_dt,
+                    int max_gt, int max_dt, long long n_ov, const double* gt_f, const int* gt_i, const double* dt_f, const int* dt_cls,
+                    const double* overlaps, const int* classes, const double* min_overlaps, int n_cls, int compute_aos,
+                    void* workspace, long long workspace_bytes, double* result, void* stream) {
     if (!gt_off || !dt_off || !ov_off || !classes || !min_overlaps || !result) return MDB_EINVAL;
     if ((n_gt > 0 && (!gt_f || !gt_i)) || (n_dt > 0 && (!dt_f || !dt_cls)) || (n_ov > 0 && !overlaps) || n_ov < 0) return MDB_EINVAL;
     const int rc = check_sizes(n_img, n_gt, n_dt, n_cls, max_gt, max_dt);
@@ -623,11 +636,31 @@ extern "C" int mdb_kitti_eval(const int* gt_off, const int* dt_off, const long l
     int* n_thr = (int*)(ws + w.n_thr);
     int* counts = (int*)(ws + w.counts);
     double* sim = (double*)(ws + w.sim);
-    clean_kernel<<<n_cls * 3, 256, 0, s>>>(gt_f, gt_i, dt_f, dt_cls, classes, n_gt, n_dt, (signed char*)(ws + w.ign_gt),
-                                           (signed char*)(ws + w.ign_dt), n_valid);
+    auto clean = by_distance ? clean_kernel<true> : clean_kernel<false>;
+    clean<<<n_cls * 3, 256, 0, s>>>(gt_f, gt_i, dt_f, dt_cls, classes, n_gt, n_dt, (signed char*)(ws + w.ign_gt),
+                                    (signed char*)(ws + w.ign_dt), n_valid);
     pass1_kernel<<<dim3((n_img + kWarps - 1) / kWarps, n_cfg), kWarps * 32, 0, s>>>(in, scores, w.P);
     thresholds_kernel<<<n_cfg, 512, 0, s>>>(scores, w.P, n_gt, n_cls, n_valid, thr, n_thr, counts);
     pass2_kernel<<<dim3((n_img * kThr + kWarps - 1) / kWarps, n_cfg), kWarps * 32, 0, s>>>(in, thr, n_thr, compute_aos, counts, sim);
     reduce_kernel<<<(n_cfg * kThr + 127) / 128, 128, 0, s>>>(n_cfg, n_img, compute_aos, n_cls, n_thr, counts, sim, result);
     return (int)cudaGetLastError();
+}
+
+}  // namespace
+
+extern "C" int mdb_kitti_eval(const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int n_gt, int n_dt,
+                              int max_gt, int max_dt, long long n_ov, const double* gt_f, const int* gt_i, const double* dt_f,
+                              const int* dt_cls, const double* overlaps, const int* classes, const double* min_overlaps, int n_cls,
+                              int compute_aos, void* workspace, long long workspace_bytes, double* result, void* stream) {
+    return kitti_eval_impl(false, gt_off, dt_off, ov_off, n_img, n_gt, n_dt, max_gt, max_dt, n_ov, gt_f, gt_i, dt_f, dt_cls, overlaps,
+                           classes, min_overlaps, n_cls, compute_aos, workspace, workspace_bytes, result, stream);
+}
+
+extern "C" int mdb_kitti_eval_distance(const int* gt_off, const int* dt_off, const long long* ov_off, int n_img, int n_gt, int n_dt,
+                                       int max_gt, int max_dt, long long n_ov, const double* gt_f, const int* gt_i, const double* dt_f,
+                                       const int* dt_cls, const double* overlaps, const int* classes, const double* min_overlaps,
+                                       int n_cls, int compute_aos, void* workspace, long long workspace_bytes, double* result,
+                                       void* stream) {
+    return kitti_eval_impl(true, gt_off, dt_off, ov_off, n_img, n_gt, n_dt, max_gt, max_dt, n_ov, gt_f, gt_i, dt_f, dt_cls, overlaps,
+                           classes, min_overlaps, n_cls, compute_aos, workspace, workspace_bytes, result, stream);
 }

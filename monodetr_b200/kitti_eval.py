@@ -2,8 +2,10 @@
 
   get_official_eval_result(gt_annos, dt_annos, current_classes, PR_detail_dict=None)
                                        lib/datasets/kitti/kitti_eval_python/eval.py:717-825
+  get_distance_eval_result(gt_annos, dt_annos, current_classes, PR_detail_dict=None)
+                                       eval.py:828-936 (AP per distance bin 0-30 / 30-50 / 50-70 m)
   do_eval(gt_annos, dt_annos, current_classes, min_overlaps, compute_aos=False, PR_detail_dict=None, DIForDIS=True)
-                                       eval.py:656-696
+                                       eval.py:656-696 (DIForDIS=False: distance bins, eval.py:85-159)
   get_label_anno(path) / get_label_annos(folder, image_ids=None)
                                        lib/datasets/kitti/kitti_eval_python/kitti_common.py:294-347
   evaluate(results_dir, label_dir, image_ids, classes, logger)
@@ -18,7 +20,7 @@ There is no CPU path: without a GPU the call raises.
 
 `GroundTruth` + `DeviceEvaluator` run the validation pass without result files: the decoded detections of each batch are
 collected into a device table (csrc/kitti_eval.cu mdb_kitti_collect_dets_f32), compacted at the end of the pass and evaluated by
-the same kernels (`eval_device_tables`).
+the same kernels (`eval_device_tables`); `DeviceEvaluator.distance_result` gives the distance-binned report of the same table.
 """
 import io
 import logging
@@ -197,19 +199,20 @@ def _check_classes(classes, min_overlaps):
     return classes, min_overlaps
 
 
-def eval_counts(gt_annos, dt_annos, classes, min_overlaps, compute_aos):
+def eval_counts(gt_annos, dt_annos, classes, min_overlaps, compute_aos, by_distance=False):
     """The device pipeline: (n_cfg, 1 + 4 * 41) fp64 table, cfg = ((metric * n_cls + m) * 3 + difficulty) * 2 + k, row =
-    [T, (tp, fp, fn, similarity) per threshold].  Six launches, one upload, one download."""
+    [T, (tp, fp, fn, similarity) per threshold].  by_distance: the third index is the distance bin (0-30, 30-50, 50-70 m) of
+    clean_data_by_distance instead of the difficulty.  Six launches, one upload, one download."""
     classes, min_overlaps = _check_classes(classes, min_overlaps)
     p = pack(gt_annos, dt_annos)
-    return eval_device_tables(_to_device(p, classes, min_overlaps), p, len(classes), compute_aos)
+    return eval_device_tables(_to_device(p, classes, min_overlaps), p, len(classes), compute_aos, by_distance)
 
 
-def eval_device_tables(d, p, n_cls, compute_aos):
+def eval_device_tables(d, p, n_cls, compute_aos, by_distance=False):
     """The counts table of `eval_counts` from tables already on the device: `d` holds the device arrays gt_off, dt_off, ov_off,
     gt_f, gt_i, dt_f, dt_cls, classes and min_overlaps, `p` the HOST sizes n_img, n_gt, n_dt, n_ov, max_gt, max_dt.  Every
     evaluation (annotation lists or the device table of `DeviceEvaluator`) launches the eval kernels here: six launches, one
-    download."""
+    download.  by_distance selects mdb_kitti_eval_distance (distance bins) over mdb_kitti_eval (difficulties)."""
     dev = d["gt_f"].device
     ov = _launch_overlaps(p, d)
     need = _lib.lib().mdb_kitti_eval_workspace_bytes(p["n_img"], p["n_gt"], p["n_dt"], n_cls, int(compute_aos))
@@ -218,7 +221,7 @@ def eval_device_tables(d, p, n_cls, compute_aos):
     ws = torch.empty(max(int(need), 1), dtype=torch.uint8, device=dev)
     n_cfg = 18 * n_cls
     result = torch.empty(n_cfg, 1 + 4 * NUM_THRESH, dtype=torch.float64, device=dev)
-    _lib.call("mdb_kitti_eval", d["gt_off"], d["dt_off"], d["ov_off"], p["n_img"], p["n_gt"], p["n_dt"], p["max_gt"], p["max_dt"],
+    _lib.call("mdb_kitti_eval_distance" if by_distance else "mdb_kitti_eval", d["gt_off"], d["dt_off"], d["ov_off"], p["n_img"], p["n_gt"], p["n_dt"], p["max_gt"], p["max_dt"],
               p["n_ov"], d["gt_f"], d["gt_i"], d["dt_f"], d["dt_cls"], ov, d["classes"], d["min_overlaps"], n_cls,
               int(compute_aos), ws, int(need), result, launches=5)
     table = result.cpu().numpy()
@@ -261,11 +264,9 @@ def _map40(prec):               # eval.py:640-644
 
 def do_eval(gt_annos, dt_annos, current_classes, min_overlaps, compute_aos=False, PR_detail_dict=None, DIForDIS=True):
     """(mAP_bbox, mAP_bev, mAP_3d, mAP_aos, mAP_bbox_R40, mAP_bev_R40, mAP_3d_R40, mAP_aos_R40), each (n_cls, 3 difficulties,
-    2 overlap sets); the aos pair is None without compute_aos.  min_overlaps (2, 3, n_cls).  All metrics and classes in one
-    device call."""
-    if not DIForDIS:
-        raise NotImplementedError("kitti_eval: the distance-binned evaluation (DIForDIS=False) is not implemented")
-    table = eval_counts(gt_annos, dt_annos, current_classes, min_overlaps, compute_aos)
+    2 overlap sets); the aos pair is None without compute_aos.  min_overlaps (2, 3, n_cls).  DIForDIS=False: the 3 distance bins
+    0-30 / 30-50 / 50-70 m (clean_data_by_distance) in place of the difficulties.  All metrics and classes in one device call."""
+    table = eval_counts(gt_annos, dt_annos, current_classes, min_overlaps, compute_aos, by_distance=not DIForDIS)
     return _aps(table, len(current_classes), compute_aos, PR_detail_dict)
 
 
@@ -297,7 +298,11 @@ def _class_codes(current_classes):
     return [NAME_TO_CLASS[c] if isinstance(c, str) else c for c in current_classes]
 
 
-def _official(gt_annos, dt_annos, current_classes, PR_detail_dict=None):
+DIFFICULTY_KEYS = ("easy", "moderate", "hard")          # ret_dict key parts of the third index: get_official_eval_result
+DISTANCE_KEYS = ("30m", "50m", "70m")                    # and get_distance_eval_result (eval.py:890-934)
+
+
+def _official(gt_annos, dt_annos, current_classes, PR_detail_dict=None, by_distance=False):
     classes = _class_codes(current_classes)
     min_overlaps = OFFICIAL_MIN_OVERLAPS[:, :, classes]
     compute_aos = False                                     # eval.py:745-751: the first image with detections decides
@@ -305,12 +310,13 @@ def _official(gt_annos, dt_annos, current_classes, PR_detail_dict=None):
         if anno["alpha"].shape[0] != 0:
             compute_aos = bool(anno["alpha"][0] != -10)
             break
-    aps = do_eval(gt_annos, dt_annos, classes, min_overlaps, compute_aos, PR_detail_dict=PR_detail_dict)
-    return _report(classes, min_overlaps, aps, compute_aos)
+    aps = do_eval(gt_annos, dt_annos, classes, min_overlaps, compute_aos, PR_detail_dict=PR_detail_dict, DIForDIS=not by_distance)
+    return _report(classes, min_overlaps, aps, compute_aos, DISTANCE_KEYS if by_distance else DIFFICULTY_KEYS)
 
 
-def _report(classes, min_overlaps, aps, compute_aos):
-    """get_official_eval_result's per-class result strings, ret_dict and first value from do_eval's arrays."""
+def _report(classes, min_overlaps, aps, compute_aos, levels=DIFFICULTY_KEYS):
+    """get_official_eval_result's (levels = DIFFICULTY_KEYS) or get_distance_eval_result's (DISTANCE_KEYS) per-class result
+    strings, ret_dict and first value from do_eval's arrays; the two reports differ only in the ret_dict keys."""
     bbox, bev, d3, aos, bbox40, bev40, d340, aos40 = aps
     texts, ret = [], {}
     for j, c in enumerate(classes):
@@ -326,12 +332,12 @@ def _report(classes, min_overlaps, aps, compute_aos):
                     text += _line(f"aos  AP:{v[j, 0, i]:.2f}, {v[j, 1, i]:.2f}, {v[j, 2, i]:.2f}")
                     if i == 0:
                         sfx = "" if tag == "AP" else "_R40"
-                        for l, diff in enumerate(("easy", "moderate", "hard")):
+                        for l, diff in enumerate(levels):
                             ret[f"{name}_aos_{diff}{sfx}"] = v[j, l, 0]
             if i == 0:
                 for sfx, curves in (("", (d3, bev, bbox)), ("_R40", (d340, bev40, bbox40))):
                     for key, v in zip(("3d", "bev", "image"), curves):
-                        for l, diff in enumerate(("easy", "moderate", "hard")):
+                        for l, diff in enumerate(levels):
                             ret[f"{name}_{key}_{diff}{sfx}"] = v[j, l, 0]
         texts.append(text)
     return texts, ret, d340[0, 1, 0], classes
@@ -342,6 +348,14 @@ def get_official_eval_result(gt_annos, dt_annos, current_classes, PR_detail_dict
     reference.  current_classes: a class code, a name ('Car', ...) or a list of them."""
     texts, ret, first, _ = _official(gt_annos, dt_annos, current_classes, PR_detail_dict)
     return "".join(texts), ret, first
+
+
+def get_distance_eval_result(gt_annos, dt_annos, current_classes, PR_detail_dict=None):
+    """(result string, dict of APs) of the distance-binned evaluation, as the reference (eval.py:828-936): the report of
+    get_official_eval_result with the bins 0-30 / 30-50 / 50-70 m in place of easy / moderate / hard, and ret_dict keys
+    `<Class>_{3d,bev,image,aos}_{30m,50m,70m}[_R40]`.  Every bin uses the hard level's occlusion / truncation / height limits."""
+    texts, ret, _, _ = _official(gt_annos, dt_annos, current_classes, PR_detail_dict, by_distance=True)
+    return "".join(texts), ret
 
 
 def evaluate(results_dir, label_dir, image_ids, classes=("Car", "Pedestrian", "Cyclist"), logger=None):
@@ -508,8 +522,9 @@ class DeviceEvaluator:
             raise ValueError("DeviceEvaluator: " + "; ".join(msg))
         return info, host
 
-    def counts_table(self):
-        """The (n_cfg, 1 + 4 * 41) counts table of eval_counts for this pass, and compute_aos."""
+    def counts_table(self, by_distance=False):
+        """The (n_cfg, 1 + 4 * 41) counts table of eval_counts for this pass (by_distance: the distance-binned one), and
+        compute_aos."""
         if self.gt is None:
             raise ValueError("DeviceEvaluator: no GroundTruth, nothing to evaluate against")
         info, _ = self._host_info(3 * self.n_img * 4)                         # the one synchronisation of the pass
@@ -527,7 +542,7 @@ class DeviceEvaluator:
              "dt_f": dt_f, "dt_cls": dt_cls, "classes": self._eval_consts[0], "min_overlaps": self._eval_consts[1]}
         with torch.cuda.device(self.device):
             _lib.call("mdb_kitti_compact_dets", dt_off, self.table_f, self.table_cls, self.n_img, self.topk, dt_f, dt_cls)
-            return eval_device_tables(d, sizes, len(self.classes), compute_aos), compute_aos
+            return eval_device_tables(d, sizes, len(self.classes), compute_aos, by_distance), compute_aos
 
     def result(self, logger=None):
         """What `evaluate` (KITTI_Dataset.eval) returns for this pass -- Car AP3d R40 at moderate difficulty, 0 when 'Car' is not
@@ -538,6 +553,18 @@ class DeviceEvaluator:
         logger.info("==> Evaluating (official) ...")
         aps = _aps(table, len(self.classes), compute_aos)
         return _log_result(logger, *_report(self.classes, self.min_overlaps, aps, compute_aos))
+
+    def distance_result(self, logger=None):
+        """What get_distance_eval_result returns for this pass's detections and `classes` -- (result string, ret_dict) -- from
+        the device table, without result files.  With a logger, each class's part of the result string is logged.  The same
+        errors as `result`."""
+        table, compute_aos = self.counts_table(by_distance=True)
+        aps = _aps(table, len(self.classes), compute_aos)
+        texts, ret, _, _ = _report(self.classes, self.min_overlaps, aps, compute_aos, DISTANCE_KEYS)
+        if logger is not None:
+            for t in texts:
+                logger.info(t)
+        return "".join(texts), ret
 
     def result_lines(self, class_names=None):
         """{image id: text of its result file} as the reference's Tester.save_results writes it, from one device->host copy."""

@@ -1,5 +1,6 @@
-"""Drop-in for the reference's lib/helpers/tester_helper.py `Tester` in the validation pass of `Trainer.train`
-(trainer_helper.py:97-100): `inference()` then `evaluate()`.
+"""Drop-in for the reference's lib/helpers/tester_helper.py `Tester`: the validation pass of `Trainer.train`
+(trainer_helper.py:97-100), `inference()` then `evaluate()`, and `test()`, which evaluates saved checkpoints (train_val.py's
+`-e` and the end of a training run).
 
 The reference decodes each batch on the host, writes one result file per image (`save_results`) and evaluates by reading
 those files and the split's label files back (`KITTI_Dataset.eval`).  Here the decoded detections of every batch stay in a
@@ -10,13 +11,17 @@ for byte as the reference writes them, from one device->host copy.
 Loader contract (the reference's): batches `(inputs, calibs, targets, info)` with `info['img_id']` and `info['img_size']`;
 `dataset.idx_list / label_dir / writelist / class_name / cls_mean_size`.  The batch's `calibs` (P2 of each image, as the
 val / test splits return them unchanged) feed the decode, instead of re-reading the calib files.
-`save_results(results)` is kept for callers that decode on their own; `test()` (checkpoint loading) is not provided.
+`save_results(results)` is kept for callers that decode on their own.
 """
 import os
+import re
 
 import torch
 
 from . import kitti_eval
+from .trainer import load_checkpoint
+
+_EPOCH_CHECKPOINT = re.compile(r"checkpoint_epoch_(\d+)\.pth")
 
 
 class Tester:
@@ -42,6 +47,43 @@ class Tester:
         self.evaluator = kitti_eval.DeviceEvaluator(gt, dataset.writelist, topk=cfg["topk"], threshold=cfg.get("threshold", 0.2),
                                                     cls_mean_size=dataset.cls_mean_size, class_names=self.class_name,
                                                     image_ids=ids, device=self.device)
+
+    def test(self):
+        """tester_helper.py:26-63: load a checkpoint of `<output_dir>` into the model, then `inference()` and `evaluate()`;
+        returns None (the AP goes to the log).  cfg['mode']:
+          'single' (or train_cfg['save_all'] false)  checkpoint_epoch_<cfg['checkpoint']>.pth when save_all, else
+                                                      checkpoint_best.pth; FileNotFoundError when it does not exist
+          'all' with save_all                         every checkpoint_epoch_<N>.pth directly in output_dir with
+                                                      N >= int(cfg['checkpoint']), in order of modification time
+        Anything else raises ValueError.  One difference from the reference in 'all' mode: it parses every `*.pth` name as
+        an epoch and so fails on checkpoint_best.pth, which the Trainer writes whenever a tester is attached; here the files
+        not named checkpoint_epoch_<N>.pth (checkpoint_best.pth, checkpoint.pth) are skipped."""
+        mode = self.cfg.get("mode")
+        if mode not in ("single", "all"):
+            raise ValueError(f"Tester.test: cfg['mode'] must be 'single' or 'all', got {mode!r}")
+        save_all = self.train_cfg["save_all"]
+        if mode == "single" or not save_all:
+            name = "checkpoint_epoch_{}.pth".format(self.cfg["checkpoint"]) if save_all else "checkpoint_best.pth"
+            path = os.path.join(self.output_dir, name)
+            if not os.path.exists(path):
+                raise FileNotFoundError(f"Tester.test: no checkpoint {path}")
+            checkpoints = [path]
+        else:
+            start_epoch = int(self.cfg["checkpoint"])
+            found = []
+            if os.path.isdir(self.output_dir):
+                for f in os.listdir(self.output_dir):
+                    m = _EPOCH_CHECKPOINT.fullmatch(f)
+                    path = os.path.join(self.output_dir, f)
+                    if m and int(m.group(1)) >= start_epoch and os.path.isfile(path):
+                        found.append((int(m.group(1)), path))
+            checkpoints = [p for _, p in sorted(found)]                # epoch order breaks ties of equal mtimes
+            checkpoints.sort(key=os.path.getmtime)
+        for path in checkpoints:
+            load_checkpoint(model=self.model, optimizer=None, filename=path, map_location=self.device, logger=self.logger)
+            self.model.to(self.device)
+            self.inference()
+            self.evaluate()
 
     def inference(self):
         torch.set_grad_enabled(False)
