@@ -34,14 +34,38 @@ def _third(a, b):
 
 
 def _solve_affine(src, dst):
-    """The 2x3 matrix M with M @ [x, y, 1] = dst for three point pairs (what cv2.getAffineTransform returns, float64)."""
-    A = np.zeros((6, 6), np.float64)
-    b = np.zeros(6, np.float64)
+    """The 2x3 matrix M with M @ [x, y, 1] = dst for three point pairs, bit for bit what cv2.getAffineTransform returns: its
+    6x6 system solved as cv2.solve(DECOMP_LU) does -- Gaussian elimination with partial pivoting (first largest |pivot|),
+    rows updated with a * (-1 / pivot), back substitution dividing by the pivot -- in fp64 without contraction.  A LAPACK
+    solve differs in the last bits, which moves the occasional PIL sample point across a truncation edge."""
+    A = [[0.0] * 6 for _ in range(6)]
+    b = [0.0] * 6
     for i in range(3):
-        A[2 * i, 0:3] = [src[i, 0], src[i, 1], 1.0]
-        A[2 * i + 1, 3:6] = [src[i, 0], src[i, 1], 1.0]
-        b[2 * i], b[2 * i + 1] = dst[i, 0], dst[i, 1]
-    return np.linalg.solve(A, b).reshape(2, 3)
+        x, y = float(src[i, 0]), float(src[i, 1])
+        A[2 * i][0:3] = [x, y, 1.0]
+        A[2 * i + 1][3:6] = [x, y, 1.0]
+        b[2 * i], b[2 * i + 1] = float(dst[i, 0]), float(dst[i, 1])
+    for i in range(6):
+        k = i
+        for j in range(i + 1, 6):
+            if abs(A[j][i]) > abs(A[k][i]):
+                k = j
+        if abs(A[k][i]) < np.finfo(np.float64).eps * 10:
+            raise np.linalg.LinAlgError("get_affine_transform: the three points are collinear")
+        A[i], A[k] = A[k], A[i]
+        b[i], b[k] = b[k], b[i]
+        d = -1.0 / A[i][i]
+        for j in range(i + 1, 6):
+            alpha = A[j][i] * d
+            for c in range(i + 1, 6):
+                A[j][c] += alpha * A[i][c]
+            b[j] += alpha * b[i]
+    for i in range(5, -1, -1):
+        s = b[i]
+        for c in range(i + 1, 6):
+            s -= A[i][c] * b[c]
+        b[i] = s / A[i][i]
+    return np.array(b, np.float64).reshape(2, 3)
 
 
 def get_affine_transform(center, scale, rot, output_size, shift=np.array([0, 0], dtype=np.float32), inv=0):
