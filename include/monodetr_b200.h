@@ -214,10 +214,11 @@ int mdb_unpack_conv_wgrads_multi_f32(int n, const float* const* dw_packed, float
 /* out[n] (+)= sum_m x[m][n]  (bias gradients) */
 int mdb_colsum_f32(const float* x, float* out, long long M, int N, int accumulate, void* stream);
 
-/* ---- Fused multi-head attention core, head_dim 32 (attention.cu) -------------------------------------
+/* ---- Fused multi-head attention core, head_dim 16, 32 or 64 (attention.cu) ------------------------------
  * Replaces the core of torch's F.multi_head_attention_forward as called at depthaware_transformer.py:456-459,
- * :496 and depth_predictor/transformer.py:59.  q[b][i][h][32] with token stride ldq floats (batch stride
- * Lq*ldq), k/v likewise (Lk*ldk, Lk*ldv), out[b][i][h*32] with token stride ldo.  key_padding_mask [B][Lk]
+ * :496 and depth_predictor/transformer.py:59.  head_dim in {16, 32, 64} (nheads 16 / 8 / 4 at d_model 256); any other
+ * value returns MDB_EUNSUPPORTED.  The scale is 1/sqrt(head_dim).  q[b][i][h][head_dim] with token stride ldq floats
+ * (batch stride Lq*ldq), k/v likewise (Lk*ldk, Lk*ldv), out[b][i][h*head_dim] with token stride ldo.  key_padding_mask [B][Lk]
  * bytes (nonzero = ignore) or NULL.  lse [B][H][Lq] is written by forward and read by backward.
  * Dropout on the probabilities: drop_p in [0,1); *seed is read on the device (CUDA-graph safe); `site`
  * decorrelates call sites.  delta_ws: B*H*Lq floats of workspace.

@@ -31,7 +31,8 @@ class TransformerEncoderLayer(nn.Module):
         qk_in = src + pos
         qk = Fn.linear(qk_in, a.in_proj_weight[:2 * c], a.in_proj_bias[:2 * c])            # fused q,k projection
         v = Fn.linear(src, a.in_proj_weight[2 * c:], a.in_proj_bias[2 * c:])
-        o = Fn.attention(qk[..., :c], qk[..., c:], v, src_key_padding_mask, a.dropout, self.training, self.site_base)
+        o = Fn.attention(qk[..., :c], qk[..., c:], v, src_key_padding_mask, a.dropout, self.training, self.site_base,
+                         a.num_heads)
         src2 = Fn.linear(o, a.out_proj.weight, a.out_proj.bias)
         src = Fn.add_layernorm(src, src2, self.norm1.weight, self.norm1.bias, self.norm1.eps, self.dropout1.p,
                                self.training, self.site_base + 1)

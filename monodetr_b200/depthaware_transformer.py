@@ -143,7 +143,7 @@ class DepthAwareDecoderLayer(nn.Module):
         a = self.cross_attn_depth
         q = Fn.linear(tgt, a.in_proj_weight[:c], a.in_proj_bias[:c])
         kv = ahead["kv"]() if "kv" in ahead else self.depth_kv(depth_pos_embed)                     # fused k,v projection
-        o = Fn.attention(q, kv[..., :c], kv[..., c:], mask_depth, a.dropout, self.training, sb)
+        o = Fn.attention(q, kv[..., :c], kv[..., c:], mask_depth, a.dropout, self.training, sb, self.nhead)
         tgt2 = Fn.linear(o, a.out_proj.weight, a.out_proj.bias)
         tgt = Fn.add_layernorm(tgt, tgt2, self.norm_depth.weight, self.norm_depth.bias, self.norm_depth.eps,
                                self.dropout_depth.p, self.training, sb + 1)
@@ -167,9 +167,9 @@ class DepthAwareDecoderLayer(nn.Module):
             g = self.group_num
             per = nq // g
             o = Fn.attention(q.reshape(B * g, per, c), k.reshape(B * g, per, c), v.reshape(B * g, per, c), None,
-                             s.dropout, True, sb + 2).reshape(B, nq, c)
+                             s.dropout, True, sb + 2, self.nhead).reshape(B, nq, c)
         else:
-            o = Fn.attention(q, k, v, None, 0.0, False, sb + 2)
+            o = Fn.attention(q, k, v, None, 0.0, False, sb + 2, self.nhead)
         tgt2 = Fn.linear(o, s.out_proj.weight, s.out_proj.bias)
         tgt = Fn.add_layernorm(tgt, tgt2, self.norm2.weight, self.norm2.bias, self.norm2.eps, self.dropout2.p, self.training, sb + 3)
         # ---- deformable cross attention over the image memory (:506-510) ---------------------------------------------
@@ -284,6 +284,9 @@ class DepthAwareDecoder(nn.Module):
         return torch.stack(intermediate), torch.stack(intermediate_refs), torch.stack(intermediate_dims), intermediate_boxes
 
 
+SUPPORTED_HEAD_DIMS = (16, 32, 64)       # head widths csrc/attention.cu is compiled for
+
+
 class DepthAwareTransformer(nn.Module):
     def __init__(self, d_model=256, nhead=8, num_encoder_layers=6, num_decoder_layers=6, dim_feedforward=1024, dropout=0.1,
                  activation="relu", return_intermediate_dec=False, num_feature_levels=4, dec_n_points=4, enc_n_points=4,
@@ -292,6 +295,10 @@ class DepthAwareTransformer(nn.Module):
         if two_stage or two_stage_dino:
             raise NotImplementedError("two_stage / two_stage_dino are not implemented: the reference itself fails with them "
                                       "(two_stage in the training forward, two_stage_dino in every forward)")
+        if d_model % nhead or d_model // nhead not in SUPPORTED_HEAD_DIMS:
+            supported = ", ".join(str(d_model // hd) for hd in sorted(SUPPORTED_HEAD_DIMS, reverse=True))
+            raise NotImplementedError(f"nheads={nhead} at hidden_dim={d_model}: the attention kernels take head widths "
+                                      f"{sorted(SUPPORTED_HEAD_DIMS)}, so nheads must be one of {supported}")
         self.d_model, self.nhead, self.group_num = d_model, nhead, group_num
         self.two_stage, self.use_dab, self.two_stage_dino = two_stage, use_dab, two_stage_dino
         self.two_stage_num_proposals = two_stage_num_proposals

@@ -302,25 +302,26 @@ def groupnorm_nhwc(x, gamma, beta, G=32, eps=1e-5, relu=False):
 # ---- attention core -----------------------------------------------------------------------------------------
 class _Attention(Function):
     @staticmethod
-    def forward(ctx, q, k, v, kpm, drop_p, site):
+    def forward(ctx, q, k, v, kpm, drop_p, site, heads):
         ctx.seed = K.seed_tensor(q.device) if drop_p > 0 else None
-        out, lse, kp = K.attention_forward(q, k, v, kpm, drop_p, site, ctx.seed)
+        out, lse, kp = K.attention_forward(q, k, v, kpm, drop_p, site, ctx.seed, heads)
         ctx.save_for_backward(q, k, v, kp, out, lse)
-        ctx.meta = (drop_p, site)
+        ctx.meta = (drop_p, site, heads)
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dout):
         q, k, v, kp, out, lse = ctx.saved_tensors
-        drop_p, site = ctx.meta
-        dq, dk, dv = K.attention_backward(q, k, v, kp, out, lse, dout, drop_p, site, ctx.seed)
-        return dq, dk, dv, None, None, None
+        drop_p, site, heads = ctx.meta
+        dq, dk, dv = K.attention_backward(q, k, v, kp, out, lse, dout, drop_p, site, ctx.seed, heads)
+        return dq, dk, dv, None, None, None, None
 
 
-def attention(q, k, v, key_padding_mask=None, drop_p=0.0, training=False, site=0):
-    """softmax(q k^T / sqrt(32)) v per head; q (B, Lq, 256), k/v (B, Lk, 256) (strided views allowed)."""
-    return _Attention.apply(q, k, v, key_padding_mask, drop_p if training else 0.0, site)
+def attention(q, k, v, key_padding_mask=None, drop_p=0.0, training=False, site=0, heads=None):
+    """softmax(q k^T / sqrt(d)) v per head, d = E / heads (16, 32 or 64; heads=None: d = 32); q (B, Lq, E), k/v (B, Lk, E)
+    (strided views allowed)."""
+    return _Attention.apply(q, k, v, key_padding_mask, drop_p if training else 0.0, site, heads)
 
 
 def msda(value, spatial_shapes, level_start_index, sampling_locations, attention_weights):

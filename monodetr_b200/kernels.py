@@ -51,11 +51,21 @@ def seed_tensor(device):
 
 
 # ---- attention ------------------------------------------------------------------------------------------
-def attention_forward(q, k, v, key_padding_mask=None, drop_p=0.0, site=0, seed=None):
-    """q (B, Lq, H*32), k/v (B, Lk, H*32): last dim contiguous, token stride arbitrary (views of packed buffers ok)."""
+def _heads(E, heads):
+    """(H, head width): heads=None means width-32 heads (H = E // 32)."""
+    if heads is None:
+        return E // 32, 32
+    if heads <= 0 or E % heads:
+        raise ValueError(f"attention: {heads} heads do not divide the embedding width {E}")
+    return heads, E // heads
+
+
+def attention_forward(q, k, v, key_padding_mask=None, drop_p=0.0, site=0, seed=None, heads=None):
+    """q (B, Lq, H*d), k/v (B, Lk, H*d) with H = heads and head width d = E / H (16, 32 or 64; heads=None: d = 32): last
+    dim contiguous, token stride arbitrary (views of packed buffers ok)."""
     B, Lq, E = q.shape
     Lk = k.shape[1]
-    H = E // 32
+    H, hd = _heads(E, heads)
     for t in (q, k, v):
         assert t.dtype == torch.float32 and t.stride(2) == 1 and t.stride(0) == t.shape[1] * t.stride(1)
     out = torch.empty((B, Lq, E), dtype=torch.float32, device=q.device)
@@ -64,22 +74,22 @@ def attention_forward(q, k, v, key_padding_mask=None, drop_p=0.0, site=0, seed=N
     if key_padding_mask is not None:
         kpm = key_padding_mask.to(torch.uint8).contiguous()
     seed = (seed if seed is not None else seed_tensor(q.device)) if drop_p > 0 else None
-    _lib.call("mdb_attention_forward_f32", q, k, v, kpm, out, lse, B, H, Lq, Lk, 32, q.stride(1), k.stride(1), v.stride(1), E,
+    _lib.call("mdb_attention_forward_f32", q, k, v, kpm, out, lse, B, H, Lq, Lk, hd, q.stride(1), k.stride(1), v.stride(1), E,
               float(drop_p), seed, site)
     return out, lse, kpm
 
 
-def attention_backward(q, k, v, kpm, out, lse, dout, drop_p=0.0, site=0, seed=None):
+def attention_backward(q, k, v, kpm, out, lse, dout, drop_p=0.0, site=0, seed=None, heads=None):
     B, Lq, E = q.shape
     Lk = k.shape[1]
-    H = E // 32
+    H, hd = _heads(E, heads)
     dout = dout.contiguous()
     dq = torch.empty((B, Lq, E), dtype=torch.float32, device=q.device)
     dk = torch.empty((B, Lk, E), dtype=torch.float32, device=q.device)
     dv = torch.empty((B, Lk, E), dtype=torch.float32, device=q.device)
     ws = torch.empty((B, H, Lq), dtype=torch.float32, device=q.device)
     seed = (seed if seed is not None else seed_tensor(q.device)) if drop_p > 0 else None
-    _lib.call("mdb_attention_backward_f32", q, k, v, kpm, out, lse, dout, ws, dq, dk, dv, B, H, Lq, Lk, 32, q.stride(1),
+    _lib.call("mdb_attention_backward_f32", q, k, v, kpm, out, lse, dout, ws, dq, dk, dv, B, H, Lq, Lk, hd, q.stride(1),
               k.stride(1), v.stride(1), E, E, E, E, float(drop_p), seed, site, launches=3)
     return dq, dk, dv
 
