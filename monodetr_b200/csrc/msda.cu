@@ -111,7 +111,8 @@ msda_fwd_vec_kernel(const float* __restrict__ value, const int64_t* __restrict__
                 const bool inside = (y > -1.f) && (x > -1.f) && (y < fH) && (x < fW);
                 const float xf = floorf(x), yf = floorf(y);
                 const int x0 = (int)xf, y0 = (int)yf;
-                const float lx = x - xf, ly = y - yf, hx = 1.f - lx, hy = 1.f - ly;
+                // off the image the weights multiply zeros, so they must stay finite (x - floor(x) is NaN for x = +-inf, NaN)
+                const float lx = inside ? x - xf : 0.f, ly = inside ? y - yf : 0.f, hx = 1.f - lx, hy = 1.f - ly;
                 const bool top = inside && (y0 >= 0), bot = inside && (y0 + 1 <= H - 1);
                 const bool lef = (x0 >= 0), rig = (x0 + 1 <= W - 1);
                 const float* p00 = vl + (y0 * W + x0) * pix;      // only dereferenced when the predicate holds
@@ -402,7 +403,8 @@ msda_bwd_vec_kernel(const float* __restrict__ value, const int64_t* __restrict__
                 const bool inside = live && (y > -1.f) && (x > -1.f) && (y < (float)H) && (x < (float)W);
                 const float xf = floorf(x), yf = floorf(y);
                 const int x0 = (int)xf, y0 = (int)yf;
-                const float lx = x - xf, ly = y - yf, hx = 1.f - lx, hy = 1.f - ly;
+                // finite weights off the image: they multiply the zero corners in ga / gx / gy (see the forward kernel)
+                const float lx = inside ? x - xf : 0.f, ly = inside ? y - yf : 0.f, hx = 1.f - lx, hy = 1.f - ly;
                 const bool top = inside && (y0 >= 0), bot = inside && (y0 + 1 <= H - 1);
                 const bool lef = (x0 >= 0), rig = (x0 + 1 <= W - 1);
                 const long long o00 = (long long)lbase + ((long long)y0 * W + x0) * pix;
