@@ -92,7 +92,7 @@ int mdb_msda_prep_backward_f32(const float* dloc, const float* dattn, const floa
                                const int64_t* spatial_shapes, int B, int Lq, int M, int L, int P, int ref_dim,
                                float* doff, float* dlogits, void* stream);
 
-/* The module's forward with the pre-processing INSIDE the sampling kernels (constant reference points; D = 32, L = 4, P = 4,
+/* The module's forward with the pre-processing INSIDE the sampling kernels (constant reference points; D = 32, L = 4, P in {2, 4, 8},
  * otherwise MDB_EUNSUPPORTED): offsets (B,Lq,M,L,P,2) and logits (B,Lq,M,L*P) are the raw projections, ref (B,Lq,L,ref_dim).
  * backward: grad_value zero-filled then accumulated; grad_offsets / grad_logits fully written. */
 int mdb_msda_fused_forward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start, const float* offsets,

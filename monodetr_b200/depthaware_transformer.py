@@ -285,6 +285,7 @@ class DepthAwareDecoder(nn.Module):
 
 
 SUPPORTED_HEAD_DIMS = (16, 32, 64)       # head widths csrc/attention.cu is compiled for
+SUPPORTED_POINTS = range(1, 9)           # sampling points per level: 2, 4 and 8 on the fused kernels, the rest on the two-step path
 
 
 class DepthAwareTransformer(nn.Module):
@@ -299,6 +300,10 @@ class DepthAwareTransformer(nn.Module):
             supported = ", ".join(str(d_model // hd) for hd in sorted(SUPPORTED_HEAD_DIMS, reverse=True))
             raise NotImplementedError(f"nheads={nhead} at hidden_dim={d_model}: the attention kernels take head widths "
                                       f"{sorted(SUPPORTED_HEAD_DIMS)}, so nheads must be one of {supported}")
+        for name, n in (("enc_n_points", enc_n_points), ("dec_n_points", dec_n_points)):
+            if not (isinstance(n, int) and n in SUPPORTED_POINTS):
+                raise NotImplementedError(f"{name}={n}: the deformable-attention kernels take {SUPPORTED_POINTS[0]} to "
+                                          f"{SUPPORTED_POINTS[-1]} sampling points per level")
         self.d_model, self.nhead, self.group_num = d_model, nhead, group_num
         self.two_stage, self.use_dab, self.two_stage_dino = two_stage, use_dab, two_stage_dino
         self.two_stage_num_proposals = two_stage_num_proposals

@@ -433,11 +433,12 @@ class _MsdaFusedSharedBoxes(Function):
         Lq, L = off.shape[1], shapes.shape[0]
         dout = dout.contiguous()
         gv, goff, glog = torch.empty_like(value), torch.empty_like(off), torch.empty_like(logits)
+        P = logits.shape[-1] // (M * L)
         part = torch.empty((B, Lq, M, L, 4), dtype=torch.float32, device=value.device)
-        _lib.call("mdb_msda_fused_backward_ref_f32", value, shapes, lsi, off, logits, refc, dout, B, S, M, D, L, Lq, 4, 6,
+        _lib.call("mdb_msda_fused_backward_ref_f32", value, shapes, lsi, off, logits, refc, dout, B, S, M, D, L, Lq, P, 6,
                   gv, goff, glog, part)
         dboxes = torch.empty((Lq, 6), dtype=torch.float32, device=value.device)
-        _lib.call("mdb_msda_ref_partials_reduce_f32", part, B, Lq, M, L, 4, 1, dboxes)
+        _lib.call("mdb_msda_ref_partials_reduce_f32", part, B, Lq, M, L, P, 1, dboxes)
         return gv, None, None, goff, glog, dboxes
 
 
@@ -445,7 +446,7 @@ def msda_shared_boxes(value, spatial_shapes, level_start_index, off, logits, box
     """MSDA with 6-d reference boxes (Lq, 6) shared by the batch and the levels (value_ratios == 1), differentiable in the boxes.
     Fused sampling kernels where they apply -- with the box partials when the boxes need a gradient, the plain fused forward
     when they do not (eval, no_grad) --; reproducible mode takes the two-step path (ordered scatter) with its box reduction."""
-    fused = (value.dtype == torch.float32 and value.shape[-1] == 32 and L == 4 and P == 4 and not os.environ.get("MDB_MSDA_UNFUSED")
+    fused = (value.dtype == torch.float32 and value.shape[-1] == 32 and L == 4 and P in FUSED_POINTS and not os.environ.get("MDB_MSDA_UNFUSED")
              and not _lib.lib().mdb_get_deterministic())
     if fused and not (boxes.requires_grad and torch.is_grad_enabled()):
         B, Lq = off.shape[0], off.shape[1]
@@ -572,16 +573,23 @@ def pos_learned(col, row, H, W):
     return _PosLearned.apply(col, row, H, W)
 
 
+def _fused_levels_points(value, shapes, logits):
+    """(L, P) of a fused call: the levels from the spatial shapes, the points from the logits' width M * L * P."""
+    L = shapes.shape[0]
+    return L, logits.shape[-1] // (value.shape[2] * L)
+
+
 def msda_fused_forward_raw(value, shapes, lsi, off, logits, refc):
     """mdb_msda_fused_forward_f32 on contiguous tensors (value (B,S,M,32), raw offsets / logits, constant reference points)."""
     B, S, M, D = value.shape
     Lq, rd = off.shape[1], refc.shape[-1]
+    L, P = _fused_levels_points(value, shapes, logits)
     out = torch.empty((B, Lq, M * D), dtype=torch.float32, device=value.device)
     from . import msda as _m
     if _m.PROBE is not None:        # bench.py: CUDA events tight around the launch (nothing else between them)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-    _lib.call("mdb_msda_fused_forward_f32", value, shapes, lsi, off, logits, refc, B, S, M, D, 4, Lq, 4, rd, out)
+    _lib.call("mdb_msda_fused_forward_f32", value, shapes, lsi, off, logits, refc, B, S, M, D, L, Lq, P, rd, out)
     if _m.PROBE is not None:
         e1.record()
         _m.PROBE.append((e0, e1, B, Lq))
@@ -591,14 +599,15 @@ def msda_fused_forward_raw(value, shapes, lsi, off, logits, refc):
 def msda_fused_backward_raw(value, shapes, lsi, off, logits, refc, dout):
     B, S, M, D = value.shape
     Lq, rd = off.shape[1], refc.shape[-1]
+    L, P = _fused_levels_points(value, shapes, logits)
     dout = dout.contiguous()
     gv, goff, glog = torch.empty_like(value), torch.empty_like(off), torch.empty_like(logits)
-    _lib.call("mdb_msda_fused_backward_f32", value, shapes, lsi, off, logits, refc, dout, B, S, M, D, 4, Lq, 4, rd, gv, goff, glog)
+    _lib.call("mdb_msda_fused_backward_f32", value, shapes, lsi, off, logits, refc, dout, B, S, M, D, L, Lq, P, rd, gv, goff, glog)
     return gv, goff, glog
 
 
 class _MsdaFused(Function):
-    """value (B,S,M,32), raw offsets (B,Lq,M*4*4*2), raw logits (B,Lq,M*16), constant reference points (B,Lq,4,rd) -> (B,Lq,M*32):
+    """value (B,S,M,32), raw offsets (B,Lq,M*4*P*2), raw logits (B,Lq,M*4*P), constant reference points (B,Lq,4,rd) -> (B,Lq,M*32):
     softmax / sampling-location pre-processing inside the sampling kernels (forward and backward)."""
 
     @staticmethod
@@ -617,8 +626,12 @@ class _MsdaFused(Function):
         return gv, None, None, goff, glog, None
 
 
+# point counts the fused kernels are compiled for (csrc/msda.cu); other counts take mdb_msda_prep_* + mdb_msda_*
+FUSED_POINTS = (2, 4, 8)
+
+
 def msda_fused_applicable(value, ref, n_levels, n_points):
-    return (value.dtype == torch.float32 and value.shape[-1] == 32 and n_levels == 4 and n_points == 4 and not ref.requires_grad
+    return (value.dtype == torch.float32 and value.shape[-1] == 32 and n_levels == 4 and n_points in FUSED_POINTS and not ref.requires_grad
             and ref.shape[-1] in (2, 6) and not os.environ.get("MDB_MSDA_UNFUSED")
             and not _lib.lib().mdb_get_deterministic())      # reproducible mode: ordered scatter of the two-step path
 
@@ -728,8 +741,8 @@ class _EncoderLayer(Function):
 
 
 def encoder_layer_fusable(layer, src, reference_points, padding_mask):
-    """The fused node covers the configuration the model runs (configs/monodetr.yaml): BF16x3 arithmetic, D = 32 x 4 levels x 4
-    points with constant reference points, no padding mask; anything else takes the separate nodes."""
+    """The fused node covers the configuration the model runs (configs/monodetr.yaml): BF16x3 arithmetic, D = 32 x 4 levels x 2, 4
+    or 8 points with constant reference points, no padding mask; anything else takes the separate nodes."""
     att = layer.self_attn
     dims_ok = all(w.shape[0] % 4 == 0 and w.shape[1] % 4 == 0 for w in (att.sampling_offsets.weight, att.attention_weights.weight,
                                                                          layer.linear1.weight, layer.linear2.weight))

@@ -74,7 +74,7 @@ class MSDeformAttn(nn.Module):
             output = Fn.msda_shared_boxes(value, input_spatial_shapes, input_level_start_index, sampling_offsets, attention_logits,
                                           reference_points, self.n_heads, self.n_levels, self.n_points)
             return Fn.linear(output, self.output_proj.weight, self.output_proj.bias)
-        # :145-155 fused: softmax over the 16 (level, point) logits and loc = ref + off / (W_l, H_l)   [2-d refs]
+        # :145-155 fused: softmax over the L*P (level, point) logits and loc = ref + off / (W_l, H_l)   [2-d refs]
         #                                                     or ref_xy + off / P * (l+r, t+b) / 2    [6-d refs]
         if Fn.msda_fused_applicable(value, reference_points, self.n_levels, self.n_points):
             # constant reference points (the encoder's pixel grid; decoder layers 1-2, whose boxes are detached): the
