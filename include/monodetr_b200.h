@@ -365,6 +365,43 @@ typedef struct MdbAdamwHyper {
  * that order and one rounding to fp32 -- the value optimizer_helper.py:122-124 computes on the host. */
 int mdb_adamw_advance(MdbAdamwHyper* hyper, void* stream);
 
+/* ---- SGD with momentum and Adam over the same flat buffers (optim.cu) -- torch.optim.SGD(momentum) / torch.optim.Adam, the
+ * reference's `sgd` / `adam` (lib/helpers/optimizer_helper.py:17-20) -- per element in the operation order of torch's
+ * multi-tensor branch.  p, g and the state buffers: n floats each, 16-byte aligned; elements [0, n_decay) get `weight_decay`
+ * (added to the gradient, as torch does), the rest 0.  No dampening, Nesterov, amsgrad or maximize.
+ * Each optimizer has its own device block, 8-byte aligned device memory owned by the caller, initialised like MdbAdamwHyper;
+ * when its address is passed as `hyper_dev` the step reads its scalars from it at run time (a captured CUDA graph then sees a
+ * new learning rate every replay) and ignores the host values. */
+typedef struct MdbSgdHyper {
+    double t;         /* steps taken with momentum buffers in place; mdb_sgd_advance adds 1.  The step with t == 1 (after the
+                       * advance) is the first: it sets buf = d instead of reading buf. */
+    double lr;
+} MdbSgdHyper;
+/* buf = first ? d : buf * momentum + d, d = g + wd * p; p -= lr * buf.  Host values: `lr` and `first_step` (non-zero: the
+ * buffers do not exist yet and are not read). */
+int mdb_sgd_step_f32(float* p, const float* g, float* buf, long long n, long long n_decay, float momentum, float weight_decay,
+                     float lr, int first_step, const MdbSgdHyper* hyper_dev, void* stream);
+/* One single-thread launch: t += 1. */
+int mdb_sgd_advance(MdbSgdHyper* hyper, void* stream);
+
+typedef struct MdbAdamHyper {
+    double t;         /* steps taken; mdb_adam_advance adds 1 */
+    double lr;
+    double beta1;
+    double beta2;
+    float neg_step;   /* written by mdb_adam_advance: (float)(-(lr / (1 - beta1^t))) */
+    float bc2_sqrt;   /* written by mdb_adam_advance: (float)sqrt(1 - beta2^t) */
+} MdbAdamHyper;
+/* m = lerp(m, g', one_minus_beta1), v = v * beta2 + one_minus_beta2 * g' * g', g' = g + wd * p;
+ * p += neg_step * m / (sqrt(v) / bc2_sqrt + eps).  neg_step and bc2_sqrt are the fp32 roundings of torch's fp64 step scalars;
+ * the one_minus_* arguments the fp32 roundings of the DOUBLE expressions 1 - beta*. */
+int mdb_adam_step_f32(float* p, const float* g, float* m, float* v, long long n, long long n_decay, float one_minus_beta1,
+                      float beta2, float one_minus_beta2, float eps, float weight_decay, float neg_step, float bc2_sqrt,
+                      const MdbAdamHyper* hyper_dev, void* stream);
+/* One single-thread launch: t += 1, then neg_step and bc2_sqrt of that t, every operation in fp64 in the order torch's Python
+ * floats take (1 - beta^t, (lr / bc1) * -1, bc2 ** 0.5) and one rounding to fp32 each. */
+int mdb_adam_advance(MdbAdamHyper* hyper, void* stream);
+
 /* ---- Inference post-process on the device (decode.cu) -- SURVEY.md 8 f3 ----
  * extract: lib/helpers/decode_helper.py:57-110 (extract_dets_from_outputs).  logits (B,Q,C), boxes (B,Q,6) cx cy l r t b,
  * dim3 (B,Q,3), depth (B,Q,2) [depth, log-variance], angle (B,Q,24).  dets (B,topk,37) = label, score, xs2d, ys2d, w, h, depth,

@@ -88,6 +88,10 @@ SIGNATURES = {
     "mdb_sum_mean_squares_backward_f32": [c_int, _PTR, _PTR, _PTR, _PTR, _PTR],
     "mdb_adamw_step_f32": [_PTR] * 4 + [ctypes.c_longlong] * 2 + [c_float] * 7 + [_PTR, _PTR],
     "mdb_adamw_advance": [_PTR, _PTR],
+    "mdb_sgd_step_f32": [_PTR] * 3 + [ctypes.c_longlong] * 2 + [c_float] * 3 + [c_int, _PTR, _PTR],
+    "mdb_sgd_advance": [_PTR, _PTR],
+    "mdb_adam_step_f32": [_PTR] * 4 + [ctypes.c_longlong] * 2 + [c_float] * 7 + [_PTR, _PTR],
+    "mdb_adam_advance": [_PTR, _PTR],
     "mdb_trainlog_push_f32": [_PTR, _PTR, c_int, _PTR, c_int, _PTR, _PTR],
     "mdb_criterion_prepare": [_PTR, c_int, c_int, _PTR, _PTR, _PTR, _PTR],
     "mdb_criterion_match_f32": [c_int] + [_PTR] * 6 + [c_int] * 5 + [c_float] * 4 + [_PTR] * 3,

@@ -1,15 +1,17 @@
-"""Optimizer of the training step (SURVEY.md 8f-2): the reference's AdamW (lib/helpers/optimizer_helper.py:30-129) as ONE
-fused kernel over flat buffers, and `build_optimizer` with the reference's signature / grouping rule (:7-27).
+"""Optimizers of the training step (SURVEY.md 8f-2): the reference's three `optimizer.type` values (lib/helpers/optimizer_helper.py:
+7-27) -- its own AdamW (:30-129), `torch.optim.SGD(momentum=0.9)` and `torch.optim.Adam` -- each as ONE fused kernel over flat
+buffers, and `build_optimizer` with the reference's signature / grouping rule.
 
 Layout.  The parameters the step updates are the gradient-receiving tensors of `FlatGradBucket` (monodetr_b200.ddp), in the
 bucket's order: weight-decay tensors first, then every tensor with 'bias' in its name (weight_decay 0 -- the reference's
 rule, :9-16).  At construction the optimizer moves those parameters INTO one flat fp32 buffer (`p.data` becomes a view of
-it; values, names, shapes and state_dict are unchanged), keeps exp_avg / exp_avg_sq as two more flat buffers, and takes the
-bucket's flat gradient buffer as `g`.  `step()` is then a single HBM-bound launch (`mdb_adamw_step_f32`, 28 bytes per
-parameter) instead of ~10 elementwise kernels per tensor; with `device_step=True` the bias-correction factor is computed
-on the device by a second, single-thread launch (`mdb_adamw_advance`) from a small device block that also holds the learning
-rate, so the whole step can live inside a CUDA graph and a learning-rate schedule still reaches every replay (`sync_hyper`).
-`state_dict()` / `load_state_dict()` speak the reference optimizer's checkpoint format.
+it; values, names, shapes and state_dict are unchanged), keeps its state (exp_avg / exp_avg_sq, or the momentum buffer) as more
+flat buffers, and takes the bucket's flat gradient buffer as `g`.  `step()` is then a single HBM-bound launch
+(`mdb_adamw_step_f32` / `mdb_adam_step_f32`, 28 bytes per parameter; `mdb_sgd_step_f32`, 20) instead of several elementwise
+kernels per tensor; with `device_step=True` the step count and the step scalars are computed on the device by a second,
+single-thread launch (`mdb_*_advance`) from a small device block that also holds the learning rate, so the whole step can live
+inside a CUDA graph and a learning-rate schedule still reaches every replay (`sync_hyper`).  `state_dict()` / `load_state_dict()`
+speak the reference optimizer's checkpoint format (torch's packed form).
 
 Parameters that never receive a gradient (SURVEY.md appendix C.2: sa_v_proj, query_scale, ref_point_head, label_enc; with
 use_dab sa_v_proj, query_scale_bbox, label_enc) are not in the bucket and are left untouched, exactly as the reference's `if p.grad is None: continue` (:95-96) leaves them.
@@ -22,19 +24,26 @@ from . import _lib
 from .ddp import FlatGradBucket
 
 
-class FusedAdamW(torch.optim.Optimizer):
-    """Same constructor arguments, `param_groups` keys and update rule as the reference's AdamW; amsgrad is not supported."""
+class _FlatOptimizer(torch.optim.Optimizer):
+    """What the three fused optimizers share: the parameters moved into one flat buffer in bucket order, state buffers of the
+    bucket's size, the reference's two groups (biases with weight_decay 0, then weights) in `param_groups`, one learning rate
+    for both, the step count (on the device with `device_step=True`, in a block whose first two doubles are t and lr),
+    `sync_hyper()` and checkpoints in torch's packed format over all named parameters.  A subclass names its state buffers
+    (`STATE`), the size of its device block in doubles (`HYPER_DOUBLES`) and implements `_launch()` and the per-parameter state
+    of its checkpoints."""
 
-    def __init__(self, model, bucket: FlatGradBucket = None, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, device_step=False):
-        if lr < 0.0 or eps < 0.0 or not (0.0 <= betas[0] < 1.0) or not (0.0 <= betas[1] < 1.0):
-            raise ValueError("invalid AdamW hyper-parameters")
+    STATE = ()
+    HYPER_DOUBLES = 2
+
+    def __init__(self, model, bucket, defaults, weight_decay, device_step):
         self.bucket = bucket if bucket is not None else FlatGradBucket(model)
         b = self.bucket
+        name = type(self).__name__
         if not b.params[0].is_cuda:
-            raise RuntimeError("FusedAdamW: CUDA parameters required (there is no CPU path)")
+            raise RuntimeError("%s: CUDA parameters required (there is no CPU path)" % name)
         nd = next(i for i, n in enumerate(b.names + ["bias"]) if "bias" in n)          # first no-decay tensor
         groups = [{"params": b.params[nd:], "weight_decay": 0}, {"params": b.params[:nd], "weight_decay": weight_decay}]
-        super().__init__([g for g in groups if g["params"]], dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False))
+        super().__init__([g for g in groups if g["params"]], defaults)
         # parameters -> views of one flat buffer, in bucket order
         self.flat_p = torch.zeros_like(b.flat)
         with torch.no_grad():
@@ -42,22 +51,18 @@ class FusedAdamW(torch.optim.Optimizer):
                 v = self.flat_p[off:off + p.numel()].view_as(p)
                 v.copy_(p)
                 p.data = v
-        self.exp_avg = torch.zeros_like(b.flat)
-        self.exp_avg_sq = torch.zeros_like(b.flat)
+        for s in self.STATE:
+            setattr(self, s, torch.zeros_like(b.flat))
         self.device_step = device_step
         self._count = 0
         # the reference optimizer's parameter numbering (optimizer_helper.py:7-16): every named parameter, biases first
         named = list(model.named_parameters())
         self._ref_groups = [[p for n, p in named if "bias" in n], [p for n, p in named if "bias" not in n]]
         if device_step:
-            # MdbAdamwHyper (include/monodetr_b200.h): t, lr, beta1, beta2 as doubles, then step_size as a float
-            self._hyper = torch.zeros(5, dtype=torch.float64, device=b.flat.device)
-            self._step_size = self._hyper.view(torch.float32)[8:9]
+            self._hyper = torch.zeros(self.HYPER_DOUBLES, dtype=torch.float64, device=b.flat.device)
             on_gpu = b.flat.device.type == "cuda"
             self._lr_host = torch.zeros(1, dtype=torch.float64, pin_memory=on_gpu)
             self._lr_uploaded, self._lr_event = None, (torch.cuda.Event() if on_gpu else None)
-            self._hyper[2:4] = torch.tensor(betas, dtype=torch.float64)
-            self.sync_hyper()
 
     @property
     def step_count(self):
@@ -75,7 +80,7 @@ class FusedAdamW(torch.optim.Optimizer):
     def _lr(self):
         lrs = {g["lr"] for g in self.param_groups}
         if len(lrs) != 1:                              # one flat update, one learning rate (the reference builds both groups alike)
-            raise ValueError("FusedAdamW: the parameter groups must share one learning rate, got %s" % sorted(lrs))
+            raise ValueError("%s: the parameter groups must share one learning rate, got %s" % (type(self).__name__, sorted(lrs)))
         return float(next(iter(lrs)))
 
     def sync_hyper(self):
@@ -88,7 +93,8 @@ class FusedAdamW(torch.optim.Optimizer):
         if lr == self._lr_uploaded:
             return
         if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
-            raise RuntimeError("FusedAdamW: the learning rate changed inside a CUDA graph capture; call sync_hyper() before capturing")
+            raise RuntimeError("%s: the learning rate changed inside a CUDA graph capture; call sync_hyper() before capturing"
+                               % type(self).__name__)
         if self._lr_event is not None:
             self._lr_event.synchronize()               # the previous upload has read the pinned word (it was issued an epoch ago)
         self._lr_host[0] = lr
@@ -108,24 +114,13 @@ class FusedAdamW(torch.optim.Optimizer):
     @torch.no_grad()
     def step(self, closure=None):
         loss = closure() if closure is not None else None
-        b = self.bucket
         self._grads_in_bucket()
-        g0 = self.param_groups[-1]                    # betas / eps are kept equal across the two groups (as the reference builds them)
-        (beta1, beta2), eps = g0["betas"], g0["eps"]
-        wd = max(g["weight_decay"] for g in self.param_groups)
-        step_dev = None
-        if self.device_step:                          # graph-safe: t, lr and the bias corrections live on the device
+        if self.device_step:
             self.sync_hyper()                         # no-op unless a scheduler wrote a new lr (an error inside a capture)
-            _lib.call("mdb_adamw_advance", self._hyper)
-            step_size, step_dev = 0.0, self._step_size
-        else:
-            self._count += 1
-            step_size = self._lr() * math.sqrt(1 - beta2 ** self._count) / (1 - beta1 ** self._count)
-        _lib.call("mdb_adamw_step_f32", self.flat_p, b.flat, self.exp_avg, self.exp_avg_sq, b.numel, b.n_decay, beta1, 1 - beta1, beta2,
-                  1 - beta2, eps, wd, step_size, step_dev)
+        self._launch(max(g["weight_decay"] for g in self.param_groups))
         return loss
 
-    # ---- checkpoints in the reference's format ---------------------------------------------------------------------------------
+    # ---- checkpoints in torch's packed format ------------------------------------------------------------------------------------
     def _ref_index(self):
         """id(parameter) -> its index in the packed state_dict of the reference's optimizer."""
         return {id(p): i for i, p in enumerate(self._ref_groups[0] + self._ref_groups[1])}
@@ -134,18 +129,23 @@ class FusedAdamW(torch.optim.Optimizer):
         """This optimizer's group behind the reference's bias / weight group (a model without biases has the weight group only)."""
         return self.param_groups[0] if is_bias and len(self.param_groups) > 1 else self.param_groups[-1]
 
+    def _views(self, off, p):
+        """(name, view in the parameter's shape) of every state buffer at one parameter."""
+        return [(s, getattr(self, s)[off:off + p.numel()].view_as(p)) for s in self.STATE]
+
+    def _param_state(self, views, step):
+        return {"step": step, **{s: v.clone() for s, v in views}}
+
     def state_dict(self):
-        """What `lib/helpers/optimizer_helper.build_optimizer(cfg, model).state_dict()` holds after the same steps: torch's packed
-        form over ALL named parameters, biases (weight_decay 0) then weights; `state[i] = {'step', 'exp_avg', 'exp_avg_sq'}`
-        (copies, in the parameter's shape) for the parameters that receive gradients, nothing for the others, and nothing at
-        all before the first step.  With `device_step=True` this reads the step count from the device (one synchronisation)."""
+        """What the reference's `build_optimizer(cfg, model).state_dict()` holds after the same steps: torch's packed form over ALL
+        named parameters, biases (weight_decay 0) then weights; per-parameter state (copies, in the parameter's shape) for the
+        parameters that receive gradients, nothing for the others, and nothing at all before the first step.  With
+        `device_step=True` this reads the step count from the device (one synchronisation)."""
         index, b, step = self._ref_index(), self.bucket, self.step_count
         state = {}
         if step > 0:
             for off, p in zip(b.offsets, b.params):
-                n = p.numel()
-                state[index[id(p)]] = {"step": step, "exp_avg": self.exp_avg[off:off + n].view_as(p).clone(),
-                                       "exp_avg_sq": self.exp_avg_sq[off:off + n].view_as(p).clone()}
+                state[index[id(p)]] = self._param_state(self._views(off, p), step)
         state = {i: state[i] for i in sorted(state)}
         groups, start = [], 0
         for is_bias, params in ((True, self._ref_groups[0]), (False, self._ref_groups[1])):
@@ -157,59 +157,200 @@ class FusedAdamW(torch.optim.Optimizer):
             groups.append(g)
         return {"state": state, "param_groups": groups}
 
+    def _check_groups(self, groups):
+        """Refuses loaded hyper-parameters the flat step does not implement."""
+
+    def _loaded_step(self, states):
+        """The one step count of a complete loaded state (`states`: one dict per gradient-receiving parameter)."""
+        steps = {int(s["step"]) for s in states}
+        if len(steps) != 1:
+            raise ValueError("%s.load_state_dict: one step count for all parameters is required, got %s"
+                             % (type(self).__name__, sorted(steps)))
+        return steps.pop()
+
+    def _after_load(self):
+        pass
+
     def load_state_dict(self, state_dict):
-        """Accepts the dict `state_dict()` returns or one saved by the reference's `AdamW` over the same model: the moments are
-        scattered into the flat buffers, the hyper-parameters (lr included, as torch does) are taken from the loaded groups, keys
-        this class does not know are kept in `param_groups` and otherwise ignored.  All parameters are updated by one kernel with
-        ONE step count, so a state whose `step` values differ between parameters, or that holds moments for only some of the
-        gradient-receiving parameters, raises ValueError."""
+        """Accepts the dict `state_dict()` returns or one saved by the reference's optimizer of the same type over the same model:
+        the state is scattered into the flat buffers, the hyper-parameters (lr included, as torch does) are taken from the loaded
+        groups, keys this class does not know are kept in `param_groups` and otherwise ignored.  All parameters are updated by one
+        kernel with ONE step count, so a state whose `step` values differ between parameters, or that holds state for only some
+        of the gradient-receiving parameters, raises ValueError."""
+        name = type(self).__name__
         groups = state_dict["param_groups"]
         if len(groups) != 2 or [len(g["params"]) for g in groups] != [len(g) for g in self._ref_groups]:
-            raise ValueError("FusedAdamW.load_state_dict: expected the reference's two groups (biases, weights) over this model's "
-                             "%d + %d parameters" % tuple(len(g) for g in self._ref_groups))
+            raise ValueError("%s.load_state_dict: expected the reference's two groups (biases, weights) over this model's "
+                             "%d + %d parameters" % ((name,) + tuple(len(g) for g in self._ref_groups)))
+        self._check_groups(groups)
         order = list(groups[0]["params"]) + list(groups[1]["params"])
         by_param = {id(p): i for p, i in zip(self._ref_groups[0] + self._ref_groups[1], order)}
         state, b = state_dict["state"], self.bucket
         have = [by_param[id(p)] in state for p in b.params]
         extra = set(state) - {by_param[id(p)] for p in b.params}
         if extra:
-            raise ValueError("FusedAdamW.load_state_dict: state for parameters that receive no gradient here: %s" % sorted(extra))
+            raise ValueError("%s.load_state_dict: state for parameters that receive no gradient here: %s" % (name, sorted(extra)))
         if any(have) and not all(have):
-            raise ValueError("FusedAdamW.load_state_dict: moments are missing for some gradient-receiving parameters")
-        steps = {int(state[by_param[id(p)]]["step"]) for p in b.params} if all(have) else {0}
-        if len(steps) != 1:
-            raise ValueError("FusedAdamW.load_state_dict: one step count for all parameters is required, got %s" % sorted(steps))
+            raise ValueError("%s.load_state_dict: moments are missing for some gradient-receiving parameters" % name)
+        step = self._loaded_step([state[by_param[id(p)]] for p in b.params]) if all(have) else 0
         with torch.no_grad():
-            self.exp_avg.zero_()
-            self.exp_avg_sq.zero_()
+            for s in self.STATE:
+                getattr(self, s).zero_()
             if all(have):
                 for off, p in zip(b.offsets, b.params):
-                    s, n = state[by_param[id(p)]], p.numel()
-                    self.exp_avg[off:off + n].view_as(p).copy_(s["exp_avg"])
-                    self.exp_avg_sq[off:off + n].view_as(p).copy_(s["exp_avg_sq"])
+                    loaded = state[by_param[id(p)]]
+                    for s, v in self._views(off, p):
+                        v.copy_(loaded[s])
         for is_bias in (True, False):
             self._own_group(is_bias).update({k: v for k, v in groups[0 if is_bias else 1].items() if k != "params"})
-        self.step_count = steps.pop()
+        self.step_count = step
+        self._after_load()
         if self.device_step:
-            self._hyper[2:4] = torch.tensor(self.param_groups[-1]["betas"], dtype=torch.float64)
             self.sync_hyper()
 
     def zero_grad(self, set_to_none=True):
         self.bucket.zero()
 
 
+class FusedAdamW(_FlatOptimizer):
+    """Same constructor arguments, `param_groups` keys and update rule as the reference's AdamW; amsgrad is not supported."""
+
+    STATE = ("exp_avg", "exp_avg_sq")
+    HYPER_DOUBLES = 5
+
+    def __init__(self, model, bucket: FlatGradBucket = None, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, device_step=False):
+        if lr < 0.0 or eps < 0.0 or not (0.0 <= betas[0] < 1.0) or not (0.0 <= betas[1] < 1.0):
+            raise ValueError("invalid AdamW hyper-parameters")
+        super().__init__(model, bucket, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False), weight_decay,
+                         device_step)
+        if device_step:
+            # MdbAdamwHyper (include/monodetr_b200.h): t, lr, beta1, beta2 as doubles, then step_size as a float
+            self._step_size = self._hyper.view(torch.float32)[8:9]
+            self._after_load()
+            self.sync_hyper()
+
+    def _launch(self, wd):
+        b = self.bucket
+        g0 = self.param_groups[-1]                    # betas / eps are kept equal across the two groups (as the reference builds them)
+        (beta1, beta2), eps = g0["betas"], g0["eps"]
+        step_dev = None
+        if self.device_step:                          # graph-safe: t, lr and the bias corrections live on the device
+            _lib.call("mdb_adamw_advance", self._hyper)
+            step_size, step_dev = 0.0, self._step_size
+        else:
+            self._count += 1
+            step_size = self._lr() * math.sqrt(1 - beta2 ** self._count) / (1 - beta1 ** self._count)
+        _lib.call("mdb_adamw_step_f32", self.flat_p, b.flat, self.exp_avg, self.exp_avg_sq, b.numel, b.n_decay, beta1, 1 - beta1, beta2,
+                  1 - beta2, eps, wd, step_size, step_dev)
+
+    def _after_load(self):
+        if self.device_step:
+            self._hyper[2:4] = torch.tensor(self.param_groups[-1]["betas"], dtype=torch.float64)
+
+
+class FusedSGD(_FlatOptimizer):
+    """The reference's `sgd`: `torch.optim.SGD(groups, lr, momentum=0.9)` (dampening 0, no Nesterov, no `maximize`) as one launch
+    over the flat buffers (`mdb_sgd_step_f32`, 20 bytes per parameter), with torch's `param_groups` keys and checkpoint format
+    (`state[i] = {'momentum_buffer'}`).  torch creates the momentum buffers on the first step (buf = d) and accumulates into
+    them afterwards; here that choice is made by the kernel, from the device block's step count with `device_step=True`, so a
+    captured step is right whether or not the buffers exist.  A state loaded with momentum buffers counts as one step taken
+    (torch's SGD keeps no step count); `step_count` counts from there."""
+
+    STATE = ("momentum_buffer",)
+    HYPER_DOUBLES = 2
+
+    def __init__(self, model, bucket: FlatGradBucket = None, lr=1e-3, momentum=0.9, weight_decay=0, device_step=False):
+        if lr < 0.0 or not momentum > 0.0 or weight_decay < 0.0:
+            raise ValueError("invalid SGD hyper-parameters (the fused step needs momentum > 0)")
+        super().__init__(model, bucket, dict(lr=lr, momentum=momentum, dampening=0, nesterov=False, maximize=False, foreach=None,
+                                             differentiable=False, fused=None), weight_decay, device_step)
+        if device_step:
+            self.sync_hyper()                         # MdbSgdHyper (include/monodetr_b200.h): t, lr as doubles
+
+    def _launch(self, wd):
+        b = self.bucket
+        momentum = self.param_groups[-1]["momentum"]
+        if self.device_step:
+            _lib.call("mdb_sgd_advance", self._hyper)
+            lr, first, hyper = 0.0, 0, self._hyper
+        else:
+            self._count += 1
+            lr, first, hyper = self._lr(), int(self._count == 1), None
+        _lib.call("mdb_sgd_step_f32", self.flat_p, b.flat, self.momentum_buffer, b.numel, b.n_decay, momentum, wd, lr, first, hyper)
+
+    def _param_state(self, views, step):
+        return {s: v.clone() for s, v in views}
+
+    def _loaded_step(self, states):
+        return 1
+
+    def _check_groups(self, groups):
+        for g in groups:
+            if g.get("dampening", 0) != 0 or g.get("nesterov", False) or g.get("maximize", False) or not g.get("momentum", 0) > 0:
+                raise ValueError("FusedSGD.load_state_dict: dampening, nesterov, maximize and momentum 0 are not supported")
+
+
+class FusedAdam(_FlatOptimizer):
+    """The reference's `adam`: `torch.optim.Adam(groups, lr)` (L2 weight decay added to the gradient; no amsgrad, `maximize` or
+    decoupled decay) as one launch over the flat buffers (`mdb_adam_step_f32`, 28 bytes per parameter), with torch's
+    `param_groups` keys and checkpoint format (`state[i] = {'step': float32 tensor, 'exp_avg', 'exp_avg_sq'}`).  The two step
+    scalars, lr / (1 - beta1^t) and sqrt(1 - beta2^t), are fp64 host values in eager mode and come from the device block with
+    `device_step=True` (`mdb_adam_advance`)."""
+
+    STATE = ("exp_avg", "exp_avg_sq")
+    HYPER_DOUBLES = 5
+
+    def __init__(self, model, bucket: FlatGradBucket = None, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, device_step=False):
+        if lr < 0.0 or eps < 0.0 or not (0.0 <= betas[0] < 1.0) or not (0.0 <= betas[1] < 1.0) or weight_decay < 0.0:
+            raise ValueError("invalid Adam hyper-parameters")
+        super().__init__(model, bucket, dict(lr=lr, betas=betas, eps=eps, amsgrad=False, maximize=False, foreach=None,
+                                             capturable=False, differentiable=False, fused=None, decoupled_weight_decay=False),
+                         weight_decay, device_step)
+        if device_step:
+            # MdbAdamHyper (include/monodetr_b200.h): t, lr, beta1, beta2 as doubles, then neg_step and bc2_sqrt as floats
+            self._scalars = self._hyper.view(torch.float32)[8:10]
+            self._after_load()
+            self.sync_hyper()
+
+    def _launch(self, wd):
+        b = self.bucket
+        g0 = self.param_groups[-1]
+        (beta1, beta2), eps = g0["betas"], g0["eps"]
+        if self.device_step:
+            _lib.call("mdb_adam_advance", self._hyper)
+            neg_step, bc2_sqrt, hyper = 0.0, 1.0, self._hyper
+        else:                                         # torch/optim/adam.py, capturable=False: Python floats
+            self._count += 1
+            t = float(self._count)
+            bc1, bc2 = 1 - beta1 ** t, 1 - beta2 ** t
+            neg_step, bc2_sqrt, hyper = (self._lr() / bc1) * -1, bc2 ** 0.5, None
+        _lib.call("mdb_adam_step_f32", self.flat_p, b.flat, self.exp_avg, self.exp_avg_sq, b.numel, b.n_decay, 1 - beta1, beta2,
+                  1 - beta2, eps, wd, neg_step, bc2_sqrt, hyper)
+
+    def _param_state(self, views, step):
+        return {"step": torch.tensor(float(step), dtype=torch.float32), **{s: v.clone() for s, v in views}}
+
+    def _check_groups(self, groups):
+        for g in groups:
+            if g.get("amsgrad", False) or g.get("maximize", False) or g.get("decoupled_weight_decay", False):
+                raise ValueError("FusedAdam.load_state_dict: amsgrad, maximize and decoupled_weight_decay are not supported")
+
+    def _after_load(self):
+        if self.device_step:
+            self._hyper[2:4] = torch.tensor(self.param_groups[-1]["betas"], dtype=torch.float64)
+
+
 def build_optimizer(cfg_optimizer, model, bucket=None):
-    """lib/helpers/optimizer_helper.py:7-27 with `adamw` served by the fused kernel; sgd / adam fall back to torch.optim with
-    the same 'bias'-in-name grouping."""
-    if cfg_optimizer["type"] == "adamw":
-        return FusedAdamW(model, bucket, lr=cfg_optimizer["lr"], weight_decay=cfg_optimizer["weight_decay"])
-    weights = [p for n, p in model.named_parameters() if "bias" not in n]
-    biases = [p for n, p in model.named_parameters() if "bias" in n]
-    groups = [{"params": biases, "weight_decay": 0}, {"params": weights, "weight_decay": cfg_optimizer["weight_decay"]}]
-    if cfg_optimizer["type"] == "sgd":
-        return torch.optim.SGD(groups, lr=cfg_optimizer["lr"], momentum=0.9)
-    if cfg_optimizer["type"] == "adam":
-        return torch.optim.Adam(groups, lr=cfg_optimizer["lr"])
+    """lib/helpers/optimizer_helper.py:7-27: `adamw`, `sgd` (momentum 0.9) and `adam` (torch's defaults otherwise), each served by
+    its fused kernel over the reference's 'bias'-in-name grouping.  Built eagerly (`device_step=False`); a loop that replays a
+    captured step constructs the class itself with `device_step=True`."""
+    kind, lr, wd = cfg_optimizer["type"], cfg_optimizer["lr"], cfg_optimizer["weight_decay"]
+    if kind == "adamw":
+        return FusedAdamW(model, bucket, lr=lr, weight_decay=wd)
+    if kind == "sgd":
+        return FusedSGD(model, bucket, lr=lr, momentum=0.9, weight_decay=wd)
+    if kind == "adam":
+        return FusedAdam(model, bucket, lr=lr, weight_decay=wd)
     raise NotImplementedError("%s optimizer is not supported" % cfg_optimizer["type"])
 
 

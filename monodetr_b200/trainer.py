@@ -5,9 +5,10 @@ printed text, log lines and checkpoint files (`checkpoint.pth`, `checkpoint_epoc
 
 Two ways to run an iteration:
 
-* Graph path -- `loss` is this package's device `SetCriterion`, `optimizer` a `FusedAdamW(device_step=True)` and the environment
-  variable MDB_NO_GRAPH is unset.  The batch is copied into static device buffers and `zero grads, forward, criterion, weighted
-  sum, backward, AdamW, loss log` is replayed as ONE CUDA graph.  The first batch of a shape runs eagerly (it warms the lazily
+* Graph path -- `loss` is this package's device `SetCriterion`, `optimizer` one of the fused optimizers of `optim`
+  (`FusedAdamW`, `FusedSGD`, `FusedAdam`) built with `device_step=True`, and the environment variable MDB_NO_GRAPH is unset.  The
+  batch is copied into static device buffers and `zero grads, forward, criterion, weighted sum, backward, optimizer step, loss
+  log` is replayed as ONE CUDA graph.  The first batch of a shape runs eagerly (it warms the lazily
   built state and is an ordinary training step), the second is captured -- capturing executes nothing -- and replayed, so every
   batch trains exactly once and the parameters follow the eager loop's trajectory.  One graph per batch shape, at most
   `MAX_GRAPHS` (the loader's short last batch is the second); further shapes run eagerly.  The loss terms are logged on the device
@@ -148,8 +149,8 @@ class Trainer(object):
         self.tester = None
 
         from .criterion import SetCriterion
-        from .optim import FusedAdamW
-        self.graph_path = (isinstance(loss, SetCriterion) and isinstance(optimizer, FusedAdamW) and optimizer.device_step
+        from .optim import FusedAdam, FusedAdamW, FusedSGD
+        self.graph_path = (isinstance(loss, SetCriterion) and isinstance(optimizer, (FusedAdamW, FusedSGD, FusedAdam)) and optimizer.device_step
                            and not os.environ.get("MDB_NO_GRAPH"))
         self._steps = {}                  # batch shape -> _CapturedStep
         self._seen = {}                   # batch shape -> batches of that shape so far
