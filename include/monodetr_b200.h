@@ -424,8 +424,8 @@ int mdb_decode_dets_f32(const float* dets, const float* img_size, const float* P
  * Predictions are passed per decoder layer (layer 0 = the final outputs, then the aux outputs), L <= MDB_CRITERION_MAX_LAYERS:
  *   logits (B,Q,C), boxes (B,Q,6), dim3 (B,Q,3), depth (B,Q,2), angle (B,Q,24), all contiguous fp32.
  * Call order: prepare -> [all-reduce `total` across ranks] -> match -> depth_map -> losses; backward: depth_map (gradient mode) and
- * losses_backward.  Nothing synchronises with the host.  Q / group <= 64, Gmax <= 64, B <= 1024 (else MDB_EUNSUPPORTED). */
-#define MDB_CRITERION_MAX_LAYERS 4
+ * losses_backward.  Nothing synchronises with the host.  Q / group <= 300, Gmax <= 64, B <= 1024 (else MDB_EUNSUPPORTED). */
+#define MDB_CRITERION_MAX_LAYERS 6
 #define MDB_CRITERION_NUM_LOSSES 10
 #define MDB_LOSS_CE 0           /* loss slots of one layer in `losses` / `grad_losses` (L, MDB_CRITERION_NUM_LOSSES) */
 #define MDB_LOSS_CLASS_ERROR 1  /* (logging only, no gradient) */

@@ -21,7 +21,10 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 
-NUM_LOSSES = 10
+NUM_LOSSES = 10                 # MDB_CRITERION_NUM_LOSSES
+MAX_LAYERS = 6                  # MDB_CRITERION_MAX_LAYERS: decoder layers (final outputs + auxiliary outputs) per call
+MAX_QUERIES = 300               # queries per group the match kernel takes (csrc/criterion.cu)
+BASE_QUERIES = 64               # queries per group a SetCriterion takes unless it is built for more (max_queries)
 (CE, CLASS_ERROR, BBOX, GIOU, CARDINALITY, DEPTH, DIM, ANGLE, CENTER, DEPTH_MAP) = range(NUM_LOSSES)
 _NAMES = {CE: "loss_ce", CLASS_ERROR: "class_error", BBOX: "loss_bbox", GIOU: "loss_giou", CARDINALITY: "cardinality_error",
           DEPTH: "loss_depth", DIM: "loss_dim", ANGLE: "loss_angle", CENTER: "loss_center", DEPTH_MAP: "loss_depth_map"}
@@ -196,9 +199,15 @@ class SetCriterion(nn.Module):
     """monodetr.py:297-532.  `targets`: the loader's padded batch dict (keys labels, boxes, boxes_3d, depth, size_3d, heading_bin,
     heading_res, mask_2d) or the list of per-image dicts `Trainer.prepare_targets` builds."""
 
-    def __init__(self, num_classes, matcher, weight_dict, focal_alpha, losses, group_num=11, depth_map_scale=(80, 24)):
+    def __init__(self, num_classes, matcher, weight_dict, focal_alpha, losses, group_num=11, depth_map_scale=(80, 24),
+                 max_queries=BASE_QUERIES):
         super().__init__()
+        if not BASE_QUERIES <= max_queries <= MAX_QUERIES:
+            raise NotImplementedError(f"SetCriterion: max_queries={max_queries}: the matcher takes {BASE_QUERIES} to {MAX_QUERIES}")
         self.num_classes = num_classes
+        # Queries per group this criterion accepts.  64 unless the model it is built for has more (build_criterion sets it from
+        # cfg["num_queries"]), so that a criterion built from the loss settings alone keeps its 64-query limit.
+        self.max_queries = max_queries
         self.matcher = matcher
         self.weight_dict = weight_dict
         self.losses = losses
@@ -221,8 +230,12 @@ class SetCriterion(nn.Module):
         tgt = pack_targets(targets, logits.device)
         group = self.group_num if self.training else 1
         layers = [outputs] + list(outputs.get("aux_outputs", []))
-        if len(layers) > 4:
-            raise ValueError("SetCriterion: at most 3 auxiliary outputs")
+        if len(layers) > MAX_LAYERS:
+            raise ValueError(f"SetCriterion: at most {MAX_LAYERS - 1} auxiliary outputs")
+        Q = logits.shape[1]
+        if Q % group == 0 and Q // group > self.max_queries:
+            raise RuntimeError(f"SetCriterion: {Q // group} queries per group, but this criterion takes at most {self.max_queries}; "
+                               "build it with build_criterion(cfg) from a model section whose num_queries covers them")
         depth_logits = outputs["pred_depth_map_logits"] if "depth_map" in self.losses else None
         preds = [l[k] for l in layers for k in _PRED_KEYS]
         losses, match = _CriterionFn.apply(self, tgt, group, depth_logits, *preds)
@@ -346,4 +359,4 @@ def build_weight_dict(cfg):
 def build_criterion(cfg):
     losses = ["labels", "boxes", "cardinality", "depths", "dims", "angles", "center", "depth_map"]        # monodetr.py:603
     return SetCriterion(cfg["num_classes"], matcher=build_matcher(cfg), weight_dict=build_weight_dict(cfg), focal_alpha=cfg["focal_alpha"],
-                        losses=losses)
+                        losses=losses, max_queries=max(BASE_QUERIES, cfg.get("num_queries", 50)))

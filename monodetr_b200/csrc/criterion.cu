@@ -4,10 +4,10 @@
 // (lib/models/monodetr/matcher.py:36-104, monodetr.py:297-532, lib/helpers/trainer_helper.py:175-186): ~40 host syncs a step.
 //
 //   prepare     compact list of the valid targets of every image from the loader's padded arrays + mask, counts, total
-//   match       one warp per (decoder layer, image, query group): cost matrix in shared memory (matcher.py:57-84) and the
-//               rectangular linear-sum-assignment by shortest augmenting paths -- the algorithm scipy.optimize.
-//               linear_sum_assignment implements (Crouse 2016) -- in fp64; writes the matched query of every target and the
-//               target class of every query
+//   match       one warp per (decoder layer, image, query group): cost matrix in dynamic shared memory, sized by the launch's
+//               queries per group and targets per image (matcher.py:57-84), and the rectangular linear-sum-assignment by
+//               shortest augmenting paths -- the algorithm scipy.optimize.linear_sum_assignment implements (Crouse 2016) -- with
+//               fp64 dual variables; writes the matched query of every target and the target class of every query
 //   depth_map   per pixel: target depth bin from the ground-truth boxes (ddn_loss.py:43-101), 81-way softmax focal loss with
 //               the one-hot + 1e-6 smoothing (focalloss.py:52-125) and the foreground / background balance (balancer.py:21-53);
 //               gradient mode writes d loss / d logits
@@ -23,12 +23,14 @@
 #include <stdint.h>
 
 #include "../../include/monodetr_b200.h"
+#include "launch.cuh"
 
 namespace {
 
 constexpr int kMaxL = MDB_CRITERION_MAX_LAYERS;
 constexpr int kNK = MDB_CRITERION_NUM_LOSSES;       // loss slots per layer (order documented in the header)
-constexpr int kMaxSide = 64;                        // queries per group and targets per image the matcher accepts
+constexpr int kMaxTargets = 64;                     // targets per image the matcher accepts (so the rows' side is at most 64)
+constexpr int kMaxQueries = 300;                    // queries per group the matcher accepts
 constexpr int kBins = 12;                           // heading bins
 
 struct LayerPtrs { const float* p[kMaxL]; };
@@ -67,21 +69,38 @@ __global__ void crit_prepare_kernel(const unsigned char* __restrict__ mask, int 
 }
 
 // ---- matcher ------------------------------------------------------------------------------------------------------------
+// Dynamic shared memory of one matching with nq queries per group and at most Gmax targets (S = max(nq, Gmax) entries per side
+// array; the rows are the smaller side, so R * Cn <= nq * Gmax):
+//   double u[S], v[S], spc[S] | float cost[nq * Gmax] | int col4row[S], row4col[S], path[S] | uchar SR[S], SC[S]
+// The cost entries are fp32 values widened to double where they are read, so storing them as float loses nothing; at
+// 300 x 64 the matrix is 75 KB.
+__host__ __device__ constexpr size_t match_smem_bytes(int nq, int Gmax) {
+    return (size_t)(nq > Gmax ? nq : Gmax) * (3 * sizeof(double) + 3 * sizeof(int) + 2) + (size_t)nq * Gmax * sizeof(float);
+}
+constexpr int kMatchMaxSmem = (int)match_smem_bytes(kMaxQueries, kMaxTargets);
+
 __global__ void __launch_bounds__(32) crit_match_kernel(LayerPtrs logits, LayerPtrs boxes, const int* __restrict__ labels,
                                                         const float* __restrict__ boxes3d, const int* __restrict__ tlist,
                                                         const int* __restrict__ count, int B, int Q, int C, int group, int Gmax,
                                                         float w_class, float w_center, float w_bbox, float w_giou,
                                                         int* __restrict__ match, int* __restrict__ tclass) {
-    __shared__ double cost[kMaxSide * kMaxSide];
-    __shared__ double u[kMaxSide], v[kMaxSide], spc[kMaxSide];
-    __shared__ int col4row[kMaxSide], row4col[kMaxSide], path[kMaxSide];
-    __shared__ unsigned char SR[kMaxSide], SC[kMaxSide];
+    extern __shared__ __align__(16) unsigned char smem[];
     const int lane = threadIdx.x;
     int p = blockIdx.x;
     const int g = p % group; p /= group;
     const int b = p % B;
     const int l = p / B;
     const int nq = Q / group, q0 = g * nq, nt = count[b];
+    const int S = nq > Gmax ? nq : Gmax;
+    double* u = reinterpret_cast<double*>(smem);
+    double* v = u + S;
+    double* spc = v + S;
+    float* cost = reinterpret_cast<float*>(spc + S);
+    int* col4row = reinterpret_cast<int*>(cost + (size_t)nq * Gmax);
+    int* row4col = col4row + S;
+    int* path = row4col + S;
+    unsigned char* SR = reinterpret_cast<unsigned char*>(path + S);
+    unsigned char* SC = SR + S;
     const float* lg = logits.p[l] + ((size_t)b * Q + q0) * C;
     const float* bx = boxes.p[l] + ((size_t)b * Q + q0) * 6;
     int* tc = tclass + ((size_t)l * B + b) * Q + q0;
@@ -109,13 +128,13 @@ __global__ void __launch_bounds__(32) crit_match_kernel(LayerPtrs logits, LayerP
         const float c_giou = -giou_pair(ax0, ay0, ax1, ay1, bx0, by0, bx1, by1);
         const float c = w_bbox * c_bbox + w_center * c_center + w_class * c_class + w_giou * c_giou;   // matcher.py:87
         const int r = rows_are_targets ? j : i, cc = rows_are_targets ? i : j;
-        cost[r * Cn + cc] = (double)c;
+        cost[r * Cn + cc] = c;
     }
-    for (int i = lane; i < kMaxSide; i += 32) { u[i] = 0.0; v[i] = 0.0; col4row[i] = -1; row4col[i] = -1; }
+    for (int i = lane; i < S; i += 32) { u[i] = 0.0; v[i] = 0.0; col4row[i] = -1; row4col[i] = -1; }
     __syncwarp();
     const double kInf = 1e300;
     for (int cur = 0; cur < R; ++cur) {
-        for (int i = lane; i < kMaxSide; i += 32) { SR[i] = 0; SC[i] = 0; spc[i] = kInf; }
+        for (int i = lane; i < S; i += 32) { SR[i] = 0; SC[i] = 0; spc[i] = kInf; }
         __syncwarp();
         double minval = 0.0;
         int i = cur, sink = -1;
@@ -125,7 +144,7 @@ __global__ void __launch_bounds__(32) crit_match_kernel(LayerPtrs logits, LayerP
             int bestj = -1, bestfree = 0;
             for (int j = lane; j < Cn; j += 32) {
                 if (SC[j]) continue;
-                const double r = minval + cost[i * Cn + j] - u[i] - v[j];
+                const double r = minval + (double)cost[i * Cn + j] - u[i] - v[j];
                 if (r < spc[j]) { spc[j] = r; path[j] = i; }
                 const double s = spc[j];
                 const int fr = row4col[j] < 0;
@@ -509,7 +528,7 @@ __global__ void __launch_bounds__(kBwdThreads) crit_losses_bwd_kernel(CritArgs a
 
 int check_common(int L, int B, int Q, int C, int group, int Gmax) {
     if (L <= 0 || L > kMaxL || B <= 0 || Q <= 0 || C <= 0 || group <= 0 || Gmax <= 0 || Q % group) return MDB_EINVAL;
-    if (Q / group > kMaxSide || Gmax > kMaxSide || B > 1024) return MDB_EUNSUPPORTED;
+    if (Q / group > kMaxQueries || Gmax > kMaxTargets || B > 1024) return MDB_EUNSUPPORTED;
     return 0;
 }
 
@@ -534,8 +553,9 @@ extern "C" int mdb_criterion_match_f32(int L, const float* const* logits, const 
         if (!logits[l] || !boxes[l]) return MDB_EINVAL;
         lp.p[l] = logits[l]; bp.p[l] = boxes[l];
     }
-    crit_match_kernel<<<L * B * group, 32, 0, (cudaStream_t)stream>>>(lp, bp, labels, boxes3d, tlist, count, B, Q, C, group, Gmax, w_class,
-                                                                      w_center, w_bbox, w_giou, match, tclass);
+    if (cudaError_t e = mdb::set_max_dynamic_smem(crit_match_kernel, kMatchMaxSmem)) return (int)e;
+    crit_match_kernel<<<L * B * group, 32, match_smem_bytes(Q / group, Gmax), (cudaStream_t)stream>>>(
+        lp, bp, labels, boxes3d, tlist, count, B, Q, C, group, Gmax, w_class, w_center, w_bbox, w_giou, match, tclass);
     return (int)cudaGetLastError();
 }
 

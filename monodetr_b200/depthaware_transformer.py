@@ -185,6 +185,12 @@ class DepthAwareDecoderLayer(nn.Module):
         return Fn.add_layernorm(tgt, tgt2, self.norm3.weight, self.norm3.bias, self.norm3.eps, self.dropout4.p, self.training, sb + 6)
 
 
+def ahead_streams(lid):
+    """Branch stream indices of decoder layer `lid`'s ahead-of-time depth key-value and value projections.  Layers 0-2 keep
+    9-11 / 12-14; deeper layers take 19 and up, clear of the neck's 15-18 and of the heads' (MonoDETR._forward)."""
+    return (9 + lid, 12 + lid) if lid < 3 else (19 + 2 * (lid - 3), 20 + 2 * (lid - 3))
+
+
 class DepthAwareDecoder(nn.Module):
     def __init__(self, decoder_layer, num_layers, return_intermediate=False, d_model=None, use_dab=False):
         super().__init__()
@@ -224,7 +230,7 @@ class DepthAwareDecoder(nn.Module):
         # GEMMs that fill the SMs the decoder's small launches leave idle).
         ahead_kv, ahead_val = [], []
         for lid, layer in enumerate(self.layers):
-            bk, bv = Fn.Branch(9 + lid, level=2), Fn.Branch(12 + lid, level=2)
+            bk, bv = (Fn.Branch(i, level=2) for i in ahead_streams(lid))
             with bk:
                 kv = layer.depth_kv(depth_pos_embed)
             with bv:
@@ -286,6 +292,9 @@ class DepthAwareDecoder(nn.Module):
 
 SUPPORTED_HEAD_DIMS = (16, 32, 64)       # head widths csrc/attention.cu is compiled for
 SUPPORTED_POINTS = range(1, 9)           # sampling points per level: 2, 4 and 8 on the fused kernels, the rest on the two-step path
+# Encoder / decoder depth: the device criterion takes at most 6 decoder layers (MDB_CRITERION_MAX_LAYERS).  Up to 6 layers the
+# dropout sites of the encoder (100 + 10 i + 0..2) and the decoder (200 + 10 i + 0..6) stay below 160 and 260: none collide.
+SUPPORTED_LAYERS = range(1, 7)
 
 
 class DepthAwareTransformer(nn.Module):
@@ -304,6 +313,17 @@ class DepthAwareTransformer(nn.Module):
             if not (isinstance(n, int) and n in SUPPORTED_POINTS):
                 raise NotImplementedError(f"{name}={n}: the deformable-attention kernels take {SUPPORTED_POINTS[0]} to "
                                           f"{SUPPORTED_POINTS[-1]} sampling points per level")
+        for name, n in (("enc_layers", num_encoder_layers), ("dec_layers", num_decoder_layers)):
+            if not (isinstance(n, int) and n in SUPPORTED_LAYERS):
+                raise NotImplementedError(f"{name}={n}: {SUPPORTED_LAYERS[0]} to {SUPPORTED_LAYERS[-1]} layers are implemented")
+        if not (isinstance(dim_feedforward, int) and dim_feedforward > 0 and dim_feedforward % 4 == 0):
+            raise NotImplementedError(f"dim_feedforward={dim_feedforward}: a positive multiple of 4 is implemented")
+        if not return_intermediate_dec:
+            raise NotImplementedError("return_intermediate_dec=False is not implemented: the reference itself fails with it (its "
+                                      "decoder then returns two values where the transformer unpacks three)")
+        if d_model != 256:
+            raise NotImplementedError(f"hidden_dim={d_model} is not implemented: the reference itself fails with it (its "
+                                      "depth_pos_embed is 256 wide and is added to a hidden_dim-wide tensor)")
         self.d_model, self.nhead, self.group_num = d_model, nhead, group_num
         self.two_stage, self.use_dab, self.two_stage_dino = two_stage, use_dab, two_stage_dino
         self.two_stage_num_proposals = two_stage_num_proposals

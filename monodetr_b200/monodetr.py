@@ -19,6 +19,15 @@ from .depth_predictor import DepthPredictor
 from .depthaware_transformer import MLP, build_depthaware_transformer, inverse_sigmoid
 
 
+MAX_QUERIES = 300               # queries per group the device matcher takes (csrc/criterion.cu)
+
+
+def head_stream(lvl):
+    """Branch stream index of decoder level `lvl`'s prediction heads: 1-3 for levels 0-2, 25 and up for deeper levels (clear of
+    the decoder's branches, depthaware_transformer.ahead_streams, and of the neck's 15-18)."""
+    return 1 + lvl if lvl < 3 else 25 + (lvl - 3)
+
+
 def _get_clones(module, N):
     return nn.ModuleList([copy.deepcopy(module) for _ in range(N)])
 
@@ -44,6 +53,8 @@ class MonoDETR(nn.Module):
                                       "(two_stage in the training forward, two_stage_dino in every forward)")
         if not with_box_refine or num_feature_levels != 4:
             raise NotImplementedError("monodetr_b200 implements with_box_refine=True and num_feature_levels=4 only")
+        if not (isinstance(num_queries, int) and 1 <= num_queries <= MAX_QUERIES):
+            raise NotImplementedError(f"num_queries={num_queries}: the device matcher takes 1 to {MAX_QUERIES} queries per group")
         self.num_queries = num_queries
         self.depthaware_transformer = depthaware_transformer
         self.depth_predictor = depth_predictor
@@ -174,7 +185,7 @@ class MonoDETR(nn.Module):
         branches = []
         for lvl in range(hs.shape[0]):
             # The heads of the three decoder levels are independent chains of small GEMMs (launch-latency bound): one stream each.
-            br = Fn.Branch(1 + lvl)
+            br = Fn.Branch(head_stream(lvl))
             with br:
                 # The reference re-evaluates bbox_embed[lvl](hs[lvl]) + inverse_sigmoid(reference) here (:216-228); that is the
                 # very tensor the decoder already formed before detaching it, so it is reused (same values, same gradients).
