@@ -71,11 +71,11 @@ __global__ void crit_prepare_kernel(const unsigned char* __restrict__ mask, int 
 // ---- matcher ------------------------------------------------------------------------------------------------------------
 // Dynamic shared memory of one matching with nq queries per group and at most Gmax targets (S = max(nq, Gmax) entries per side
 // array; the rows are the smaller side, so R * Cn <= nq * Gmax):
-//   double u[S], v[S], spc[S] | float cost[nq * Gmax] | int col4row[S], row4col[S], path[S] | uchar SR[S], SC[S]
+//   double u[S], v[S], spc[S] | float cost[nq * Gmax] | int col4row[S], row4col[S], path[S], remaining[S] | uchar SR[S], SC[S]
 // The cost entries are fp32 values widened to double where they are read, so storing them as float loses nothing; at
 // 300 x 64 the matrix is 75 KB.
 __host__ __device__ constexpr size_t match_smem_bytes(int nq, int Gmax) {
-    return (size_t)(nq > Gmax ? nq : Gmax) * (3 * sizeof(double) + 3 * sizeof(int) + 2) + (size_t)nq * Gmax * sizeof(float);
+    return (size_t)(nq > Gmax ? nq : Gmax) * (3 * sizeof(double) + 4 * sizeof(int) + 2) + (size_t)nq * Gmax * sizeof(float);
 }
 constexpr int kMatchMaxSmem = (int)match_smem_bytes(kMaxQueries, kMaxTargets);
 
@@ -99,7 +99,8 @@ __global__ void __launch_bounds__(32) crit_match_kernel(LayerPtrs logits, LayerP
     int* col4row = reinterpret_cast<int*>(cost + (size_t)nq * Gmax);
     int* row4col = col4row + S;
     int* path = row4col + S;
-    unsigned char* SR = reinterpret_cast<unsigned char*>(path + S);
+    int* remaining = path + S;
+    unsigned char* SR = reinterpret_cast<unsigned char*>(remaining + S);
     unsigned char* SC = SR + S;
     const float* lg = logits.p[l] + ((size_t)b * Q + q0) * C;
     const float* bx = boxes.p[l] + ((size_t)b * Q + q0) * 6;
@@ -108,8 +109,8 @@ __global__ void __launch_bounds__(32) crit_match_kernel(LayerPtrs logits, LayerP
     for (int i = lane; i < nq; i += 32) tc[i] = C;                  // "no object"
     for (int j = lane; j < Gmax; j += 32) mt[j] = -1;
     if (nt == 0) return;
-    // rows = the smaller side (as scipy transposes when there are more rows than columns)
-    const bool rows_are_targets = nt <= nq;
+    // rows = the smaller side: scipy transposes the (query x target) matrix only when it has more rows than columns
+    const bool rows_are_targets = nt < nq;
     const int R = rows_are_targets ? nt : nq, Cn = rows_are_targets ? nq : nt;
     for (int e = lane; e < nq * nt; e += 32) {
         const int i = e / nt, j = e - i * nt;                        // query i, target j
@@ -133,33 +134,42 @@ __global__ void __launch_bounds__(32) crit_match_kernel(LayerPtrs logits, LayerP
     for (int i = lane; i < S; i += 32) { u[i] = 0.0; v[i] = 0.0; col4row[i] = -1; row4col[i] = -1; }
     __syncwarp();
     const double kInf = 1e300;
+    // Ties are broken as scipy's augmenting_path breaks them, so that equal-cost problems get scipy's assignment: the
+    // unvisited columns are scanned in the order of `remaining` (reversed at first; a picked column is replaced by the last
+    // entry), and a column of the same reduced cost displaces the current pick only if it is free.  The pick is therefore
+    // the lowest reduced cost; among ties the last free column in scan order, or the first one if none is free.
     for (int cur = 0; cur < R; ++cur) {
         for (int i = lane; i < S; i += 32) { SR[i] = 0; SC[i] = 0; spc[i] = kInf; }
+        for (int k = lane; k < Cn; k += 32) remaining[k] = Cn - 1 - k;
         __syncwarp();
         double minval = 0.0;
-        int i = cur, sink = -1;
+        int i = cur, sink = -1, nrem = Cn;
         while (sink < 0) {
             if (lane == 0) SR[i] = 1;
             double best = kInf;
-            int bestj = -1, bestfree = 0;
-            for (int j = lane; j < Cn; j += 32) {
-                if (SC[j]) continue;
+            int bestk = -1, bestj = -1, bestfree = 0;
+            for (int k = lane; k < nrem; k += 32) {                   // k rises along a lane's scan: scipy's rule applies as is
+                const int j = remaining[k];
                 const double r = minval + (double)cost[i * Cn + j] - u[i] - v[j];
                 if (r < spc[j]) { spc[j] = r; path[j] = i; }
                 const double s = spc[j];
                 const int fr = row4col[j] < 0;
-                if (s < best || (s == best && fr > bestfree)) { best = s; bestj = j; bestfree = fr; }
+                if (s < best || (s == best && fr)) { best = s; bestk = k; bestj = j; bestfree = fr; }
             }
+            // the lanes' picks ordered by (cost, free beats taken, free: later position first, taken: earlier position first)
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
                 const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-                const int oj = __shfl_xor_sync(0xffffffffu, bestj, o), of = __shfl_xor_sync(0xffffffffu, bestfree, o);
-                const bool take = oj >= 0 && (bestj < 0 || ob < best || (ob == best && (of > bestfree || (of == bestfree && oj < bestj))));
-                if (take) { best = ob; bestj = oj; bestfree = of; }
+                const int ok = __shfl_xor_sync(0xffffffffu, bestk, o), oj = __shfl_xor_sync(0xffffffffu, bestj, o);
+                const int of = __shfl_xor_sync(0xffffffffu, bestfree, o);
+                const bool tie_take = (of || bestfree) ? (of && (!bestfree || ok > bestk)) : ok < bestk;
+                const bool take = ok >= 0 && (bestk < 0 || ob < best || (ob == best && tie_take));
+                if (take) { best = ob; bestk = ok; bestj = oj; bestfree = of; }
             }
-            if (bestj < 0 || !(best < kInf)) { sink = -2; break; }      // infeasible (NaN / inf costs): leave unmatched
+            if (bestk < 0 || !(best < kInf)) { sink = -2; break; }      // infeasible (NaN / inf costs): leave unmatched
             minval = best;
-            if (lane == 0) SC[bestj] = 1;
+            if (lane == 0) { SC[bestj] = 1; remaining[bestk] = remaining[nrem - 1]; }
+            --nrem;
             if (row4col[bestj] < 0) sink = bestj; else i = row4col[bestj];
             __syncwarp();
         }
@@ -220,9 +230,11 @@ __global__ void crit_depth_map_kernel(const float* __restrict__ logits, long lon
     for (int k = lane; k < nt; k += 32) {
         const int t = tlist[b * Gmax + k];
         const float* bb = boxes2d + ((size_t)b * Gmax + t) * 4;
-        const float cx = bb[0] * sx, cy = bb[1] * sy, w = bb[2] * sx, h = bb[3] * sy;          // monodetr.py:462-463
-        const long long u1 = (long long)floorf(cx - 0.5f * w), v1 = (long long)floorf(cy - 0.5f * h);
-        const long long u2 = (long long)ceilf(cx + 0.5f * w), v2 = (long long)ceilf(cy + 0.5f * h);
+        // monodetr.py:462-463 rounds the scaled box before box_cxcywh_to_xyxy: the explicit roundings keep nvcc from
+        // contracting bb[0] * sx into the subtraction, which moves a box edge that lies on a pixel boundary by one pixel
+        const float cx = __fmul_rn(bb[0], sx), cy = __fmul_rn(bb[1], sy), hw = 0.5f * __fmul_rn(bb[2], sx), hh = 0.5f * __fmul_rn(bb[3], sy);
+        const long long u1 = (long long)floorf(__fsub_rn(cx, hw)), v1 = (long long)floorf(__fsub_rn(cy, hh));
+        const long long u2 = (long long)ceilf(__fadd_rn(cx, hw)), v2 = (long long)ceilf(__fadd_rn(cy, hh));
         if (in_py_slice(y, v1, v2, H) && in_py_slice(x, u1, u2, W)) {
             const float dk = depth[b * Gmax + t];
             d = fg ? fminf(d, dk) : dk;
@@ -235,7 +247,8 @@ __global__ void crit_depth_map_kernel(const float* __restrict__ logits, long lon
         const bool of = __shfl_xor_sync(0xffffffffu, (int)fg, o) != 0;
         if (of) { d = fg ? fminf(d, od) : od; fg = true; }
     }
-    // LID bin (ddn_loss.py:84-98)
+    // LID bin (ddn_loss.py:84-98).  d - dmin, * 8, / bin_size, + 1 and sqrtf round one by one in the SASS; only
+    // -0.5 + 0.5 * sqrt(...) is contracted into an FFMA, and 0.5 * sqrt(...) is exact, so (int)idxf sees the reference's value.
     const float bin_size = (float)(2.0 * ((double)dmax - (double)dmin) / ((double)nb * (1.0 + (double)nb)));
     const float idxf = -0.5f + 0.5f * sqrtf(1.f + 8.f * (d - dmin) / bin_size);
     int target = nb;

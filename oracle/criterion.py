@@ -93,10 +93,9 @@ def sigmoid_focal_loss(inputs, targets, num_boxes, alpha=0.25, gamma=2):
     return loss.mean(1).sum() / num_boxes
 
 
-def ddn_loss(depth_logits, gt_boxes2d, num_gt_per_img, gt_center_depth, alpha=0.25, gamma=2.0, fg_weight=13, bg_weight=1,
-             depth_min=1e-3, depth_max=60, num_bins=80):
-    B, _, H, W = depth_logits.shape
-    depth_maps = torch.zeros((B, H, W), dtype=depth_logits.dtype)
+def ddn_target(gt_boxes2d, num_gt_per_img, gt_center_depth, B, H, W, depth_min=1e-3, depth_max=60, num_bins=80):
+    """(B, H, W) LID bin of every pixel and its foreground mask, formed in the dtype of the boxes and depths."""
+    depth_maps = torch.zeros((B, H, W), dtype=gt_center_depth.dtype)
     gt_boxes2d = gt_boxes2d.clone()
     gt_boxes2d[:, :2] = torch.floor(gt_boxes2d[:, :2])
     gt_boxes2d[:, 2:] = torch.ceil(gt_boxes2d[:, 2:])
@@ -114,7 +113,15 @@ def ddn_loss(depth_logits, gt_boxes2d, num_gt_per_img, gt_center_depth, alpha=0.
     idx = -0.5 + 0.5 * torch.sqrt(1 + 8 * (depth_maps - depth_min) / bin_size)
     bad = (idx < 0) | (idx > num_bins) | (~torch.isfinite(idx))
     idx[bad] = num_bins
-    target = idx.type(torch.int64)
+    return idx.type(torch.int64), fg
+
+
+def ddn_loss(depth_logits, gt_boxes2d, num_gt_per_img, gt_center_depth, alpha=0.25, gamma=2.0, fg_weight=13, bg_weight=1,
+             depth_min=1e-3, depth_max=60, num_bins=80, per_pixel=False):
+    """The depth-map loss; with per_pixel, also the (B, H, W) weighted loss of every pixel.  The target bins are formed in the
+    dtype of the boxes and depths (ddn_target), the focal loss in that of the logits."""
+    B, _, H, W = depth_logits.shape
+    target, fg = ddn_target(gt_boxes2d, num_gt_per_img, gt_center_depth, B, H, W, depth_min, depth_max, num_bins)
     soft, logsoft = F.softmax(depth_logits, dim=1), F.log_softmax(depth_logits, dim=1)
     onehot = torch.zeros_like(depth_logits).scatter_(1, target.unsqueeze(1), 1.0) + 1e-6
     focal = -alpha * torch.pow(-soft + 1.0, gamma) * logsoft
@@ -122,21 +129,25 @@ def ddn_loss(depth_logits, gt_boxes2d, num_gt_per_img, gt_center_depth, alpha=0.
     weights = fg_weight * fg + bg_weight * (~fg)
     loss = loss * weights
     npix = fg.sum() + (~fg).sum()
-    return loss[fg].sum() / npix + loss[~fg].sum() / npix
+    total = loss[fg].sum() / npix + loss[~fg].sum() / npix
+    return (total, loss) if per_pixel else total
 
 
 def _src_idx(indices):
     return (torch.cat([torch.full_like(s, i) for i, (s, _) in enumerate(indices)]), torch.cat([s for s, _ in indices]))
 
 
-def layer_losses(out, targets, indices, num_boxes, num_classes=3, focal_alpha=0.25, log=True, depth_map=True, map_scale=(80, 24)):
+def layer_losses(out, targets, indices, num_boxes, num_classes=3, focal_alpha=0.25, log=True, depth_map=True, map_scale=(80, 24),
+                 corner_dtype=None):
+    """corner_dtype: round the predicted box corners to this dtype (keeping their gradient), as a kernel in that precision
+    forms them, so that GIoU's max / min and clamp take the same branches in a higher-precision run."""
     L = {}
     idx = _src_idx(indices)
     logits = out["pred_logits"]
     tco = torch.cat([t["labels"][J] for t, (_, J) in zip(targets, indices)])
     tc = torch.full(logits.shape[:2], num_classes, dtype=torch.int64)
     tc[idx] = tco.long()
-    onehot = torch.zeros(logits.shape[0], logits.shape[1], logits.shape[2] + 1).scatter_(2, tc.unsqueeze(-1), 1)[:, :, :-1]
+    onehot = torch.zeros(logits.shape[0], logits.shape[1], logits.shape[2] + 1, dtype=logits.dtype).scatter_(2, tc.unsqueeze(-1), 1)[:, :, :-1]
     L["loss_ce"] = sigmoid_focal_loss(logits, onehot, num_boxes, alpha=focal_alpha, gamma=2) * logits.shape[1]
     if log:
         if tco.numel() == 0:
@@ -147,7 +158,10 @@ def layer_losses(out, targets, indices, num_boxes, num_classes=3, focal_alpha=0.
     tb = torch.cat([t["boxes_3d"][i] for t, (_, i) in zip(targets, indices)], dim=0)
     sb = out["pred_boxes"][idx]
     L["loss_bbox"] = F.l1_loss(sb[:, 2:6], tb[:, 2:6], reduction="none").sum() / num_boxes
-    L["loss_giou"] = (1 - torch.diag(generalized_box_iou(cxcylrtb_to_xyxy(sb), cxcylrtb_to_xyxy(tb)))).sum() / num_boxes
+    sxy = cxcylrtb_to_xyxy(sb)
+    if corner_dtype is not None:
+        sxy = sxy + (sxy.to(corner_dtype).to(sxy.dtype) - sxy).detach()
+    L["loss_giou"] = (1 - torch.diag(generalized_box_iou(sxy, cxcylrtb_to_xyxy(tb)))).sum() / num_boxes
     lens = torch.as_tensor([len(t["labels"]) for t in targets])
     card = (logits.argmax(-1) != logits.shape[-1] - 1).sum(1)
     L["cardinality_error"] = F.l1_loss(card.float(), lens.float())
@@ -164,14 +178,15 @@ def layer_losses(out, targets, indices, num_boxes, num_classes=3, focal_alpha=0.
     hb = torch.cat([t["heading_bin"][i] for t, (_, i) in zip(targets, indices)], dim=0).view(-1).long()
     hr = torch.cat([t["heading_res"][i] for t, (_, i) in zip(targets, indices)], dim=0).view(-1)
     cls_loss = F.cross_entropy(ha[:, 0:12], hb, reduction="none")
-    oh = torch.zeros(hb.shape[0], 12).scatter_(dim=1, index=hb.view(-1, 1), value=1)
+    oh = torch.zeros(hb.shape[0], 12, dtype=ha.dtype).scatter_(dim=1, index=hb.view(-1, 1), value=1)
     reg_loss = F.l1_loss(torch.sum(ha[:, 12:24] * oh, 1), hr, reduction="none")
     L["loss_angle"] = (cls_loss + reg_loss).sum() / num_boxes
     L["loss_center"] = F.l1_loss(sb[:, 0:2], tb[:, 0:2], reduction="none").sum() / num_boxes
     if depth_map:
         n = [len(t["boxes"]) for t in targets]
         sx, sy = map_scale
-        boxes2d = cxcywh_to_xyxy(torch.cat([t["boxes"] for t in targets], dim=0) * torch.tensor([sx, sy, sx, sy], dtype=torch.float32))
+        b2 = torch.cat([t["boxes"] for t in targets], dim=0)
+        boxes2d = cxcywh_to_xyxy(b2 * torch.tensor([sx, sy, sx, sy], dtype=b2.dtype))
         L["loss_depth_map"] = ddn_loss(out["pred_depth_map_logits"], boxes2d, n, torch.cat([t["depth"] for t in targets], dim=0).squeeze(dim=1))
     return L
 
