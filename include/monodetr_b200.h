@@ -211,6 +211,40 @@ int mdb_pack_conv_weights_multi_f32(int n, const float* const* w_oihw, const flo
                                     const int* O, const int* I, const int* taps, void* stream);
 int mdb_unpack_conv_wgrads_multi_f32(int n, const float* const* dw_packed, float* const* dw_oihw, const int* O, const int* I,
                                      const int* taps, void* stream);
+/* Grouped convolutions (torch.nn.Conv2d's `groups`; ResNeXt's 3x3 conv2): kh == kw == 3, Cin == Cout == C, C % 128 == 0 and
+ * C / groups dividing 128, with the dilation rules of the *_dilated calls (pad % dilation == 0 for the weight gradient); any
+ * other geometry returns MDB_EUNSUPPORTED.  Weights are band-local: row r (an output channel in wf, an input channel in the
+ * transposed wd) holds the 128 channels of r's 128-channel band, zero outside r's group -- fp32 [9][C][128], or pre-split
+ * bf16 [9][C][4][hi 32 | lo 32] (bf16 elements: 9*C*256 each) -- written from OIHW (C, C/groups, 3, 3) weights by the pack
+ * calls (scale folded as in mdb_pack_gemm_weights_bf16x3; the fp32 pack rounds to nearest TF32 in precision mode 0).  Each
+ * output tile of 128 channels reduces over its own band only (9 x 128 per pixel).  The _f32 forward / dgrad run 3xTF32 in
+ * precision mode 2, like the dense _f32 calls; flags, residual, relu_mask, reproducibility and batch independence are those
+ * of the dense calls; the forward never splits K and needs no workspace.  The weight gradient writes the band-local
+ * dw_band[9][C][128] (+)= rowscale[co] * sum dy * x over each 128 x 128 diagonal block (zero-filled first unless accumulate):
+ * the in-group entries and, between them, the products across the band's other groups, which the grouped convolution does
+ * not have; mdb_unpack_conv_wgrads_grouped_multi_f32 keeps the in-group entries as OIHW.  Array arguments are HOST arrays (one launch
+ * per 64 tensors); scale and wd may be NULL or hold NULL entries. */
+int mdb_conv2d_forward_grouped_f32(const float* x, const float* w_band, const float* bias, const float* residual, float* y, int B,
+                                   int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation, int groups,
+                                   int flags, void* stream);
+int mdb_conv2d_forward_grouped_bf16x3(const float* x, const void* w_band, const float* bias, const float* residual, float* y,
+                                      int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                      int groups, int flags, void* stream);
+int mdb_conv2d_dgrad_grouped_f32(const float* dy, const float* w_band_t, const float* residual, const float* relu_mask, float* dx,
+                                 int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation, int groups,
+                                 int flags, void* stream);
+int mdb_conv2d_dgrad_grouped_bf16x3(const float* dy, const void* w_band_t, const float* residual, const float* relu_mask,
+                                    float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                    int dilation, int groups, int flags, void* stream);
+int mdb_conv2d_wgrad_grouped_f32(const float* dy, const float* x, const float* rowscale /*[C]|NULL*/, float* dw_band, int B, int H,
+                                 int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation, int groups,
+                                 int accumulate, void* stream);
+int mdb_pack_conv_weights_grouped_multi_f32(int n, const float* const* w_oihw, const float* const* scale, float* const* wf,
+                                            float* const* wd, const int* C, const int* groups, void* stream);
+int mdb_pack_conv_weights_grouped_multi_bf16x3(int n, const float* const* w_oihw, const float* const* scale, void* const* wf,
+                                               void* const* wd, const int* C, const int* groups, void* stream);
+int mdb_unpack_conv_wgrads_grouped_multi_f32(int n, const float* const* dw_band, float* const* dw_oihw, const int* C,
+                                             const int* groups, void* stream);
 /* out[n] (+)= sum_m x[m][n]  (bias gradients) */
 int mdb_colsum_f32(const float* x, float* out, long long M, int N, int accumulate, void* stream);
 

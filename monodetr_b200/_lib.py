@@ -50,6 +50,14 @@ SIGNATURES = {
     "mdb_unpack_conv_wgrad_f32": [_PTR] * 2 + [c_int] * 4 + [_PTR],
     "mdb_pack_conv_weights_multi_f32": [c_int] + [_PTR] * 6 + [_PTR],
     "mdb_unpack_conv_wgrads_multi_f32": [c_int] + [_PTR] * 5 + [_PTR],
+    "mdb_conv2d_forward_grouped_f32": [_PTR] * 5 + [c_int] * 12 + [_PTR],
+    "mdb_conv2d_forward_grouped_bf16x3": [_PTR] * 5 + [c_int] * 12 + [_PTR],
+    "mdb_conv2d_dgrad_grouped_f32": [_PTR] * 5 + [c_int] * 12 + [_PTR],
+    "mdb_conv2d_dgrad_grouped_bf16x3": [_PTR] * 5 + [c_int] * 12 + [_PTR],
+    "mdb_conv2d_wgrad_grouped_f32": [_PTR] * 4 + [c_int] * 12 + [_PTR],
+    "mdb_pack_conv_weights_grouped_multi_f32": [c_int] + [_PTR] * 6 + [_PTR],
+    "mdb_pack_conv_weights_grouped_multi_bf16x3": [c_int] + [_PTR] * 6 + [_PTR],
+    "mdb_unpack_conv_wgrads_grouped_multi_f32": [c_int] + [_PTR] * 4 + [_PTR],
     "mdb_colsum_f32": [_PTR] * 2 + [ctypes.c_longlong, c_int, c_int, _PTR],
     "mdb_attention_forward_f32": [_PTR] * 6 + [c_int] * 9 + [c_float, _PTR, ctypes.c_ulonglong, _PTR],
     "mdb_attention_backward_f32": [_PTR] * 11 + [c_int] * 12 + [c_float, _PTR, ctypes.c_ulonglong, _PTR],

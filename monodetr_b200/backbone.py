@@ -1,13 +1,15 @@
 """ResNet backbones on the sm_90a kernels -- host-side mirror of the reference's
 lib/models/monodetr/backbone.py (FrozenBatchNorm2d :27-64, BackboneBase :67-90, Backbone :93-108, Joiner
-:111-126, build_backbone :129-135) with torchvision's bottleneck ResNets (resnet50 / 101 / 152, v1.5: stride on the 3x3;
-optionally with layer4's stride replaced by dilation 2, the "DC5" variant) restated as parameter containers with the same
-state_dict keys (`backbone.0.body.*`).
+:111-126, build_backbone :129-135) with torchvision's bottleneck ResNets (resnet50 / 101 / 152, the ResNeXts resnext50_32x4d / resnext101_32x8d /
+resnext101_64x4d and the wide ResNets wide_resnet50_2 / 101_2; v1.5: stride on the 3x3; optionally with layer4's stride
+replaced by dilation 2, the "DC5" variant) restated as parameter containers with the same state_dict keys
+(`backbone.0.body.*`).
 
 Execution is ONE hand-scheduled autograd Function (no cuDNN, no per-layer autograd nodes):
   * conv1 7x7/2 + FrozenBN + ReLU and max-pool: dedicated forward-only kernels (conv1/layer1 are frozen, :71-73);
   * every other conv is the wgmma implicit-GEMM kernel with FrozenBN folded in: scale into the packed weights,
-    shift as the epilogue bias, ReLU / residual-add+ReLU in the epilogue, activations NHWC;
+    shift as the epilogue bias, ReLU / residual-add+ReLU in the epilogue, activations NHWC; a ResNeXt's grouped 3x3
+    conv2 runs the channel-banded form of that kernel (tc.conv2d_* with groups);
   * backward: dgrad kernels apply the previous ReLU's mask (and add the identity-branch gradient) in their
     epilogue, wgrad kernels multiply by the BN scale per output row; layer1 and the stem get no backward.
 """
@@ -24,6 +26,15 @@ from .position_encoding import build_position_encoding
 # (stage, planes, stride) of torchvision's ResNet, and the blocks per stage of each bottleneck depth it builds
 _STAGES = [("layer1", 64, 1), ("layer2", 128, 2), ("layer3", 256, 2), ("layer4", 512, 2)]
 RESNET_DEPTHS = {"resnet50": (3, 4, 6, 3), "resnet101": (3, 4, 23, 3), "resnet152": (3, 8, 36, 3)}
+# torchvision's ResNeXts and wide ResNets by name: (blocks per stage, groups, width_per_group); the 3x3 of a block with
+# `planes` has width = planes * width_per_group / 64 * groups channels
+RESNEXT_BODIES = {
+    "resnext50_32x4d": (RESNET_DEPTHS["resnet50"], 32, 4),
+    "resnext101_32x8d": (RESNET_DEPTHS["resnet101"], 32, 8),
+    "resnext101_64x4d": (RESNET_DEPTHS["resnet101"], 64, 4),
+    "wide_resnet50_2": (RESNET_DEPTHS["resnet50"], 1, 128),
+    "wide_resnet101_2": (RESNET_DEPTHS["resnet101"], 1, 128),
+}
 
 
 class FrozenBatchNorm2d(nn.Module):
@@ -46,8 +57,9 @@ class FrozenBatchNorm2d(nn.Module):
         return scale.contiguous(), (self.bias - self.running_mean * scale).contiguous()
 
 
-def _conv(cin, cout, k, stride=1, dilation=1):
-    m = nn.Conv2d(cin, cout, k, stride=stride, padding=dilation * (k // 2), dilation=dilation, bias=False)   # parameter container only
+def _conv(cin, cout, k, stride=1, dilation=1, groups=1):
+    m = nn.Conv2d(cin, cout, k, stride=stride, padding=dilation * (k // 2), dilation=dilation, groups=groups,
+                  bias=False)   # parameter container only
     nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
     return m
 
@@ -55,27 +67,30 @@ def _conv(cin, cout, k, stride=1, dilation=1):
 class Bottleneck(nn.Module):
     expansion = 4
 
-    def __init__(self, inplanes, planes, stride, downsample, dilation=1):
+    def __init__(self, inplanes, planes, stride, downsample, dilation=1, groups=1, width_per_group=64):
         super().__init__()
-        self.conv1 = _conv(inplanes, planes, 1)
-        self.bn1 = FrozenBatchNorm2d(planes)
-        self.conv2 = _conv(planes, planes, 3, stride, dilation)
-        self.bn2 = FrozenBatchNorm2d(planes)
-        self.conv3 = _conv(planes, planes * 4, 1)
+        width = int(planes * (width_per_group / 64.0)) * groups      # torchvision's Bottleneck
+        self.conv1 = _conv(inplanes, width, 1)
+        self.bn1 = FrozenBatchNorm2d(width)
+        self.conv2 = _conv(width, width, 3, stride, dilation, groups)
+        self.bn2 = FrozenBatchNorm2d(width)
+        self.conv3 = _conv(width, planes * 4, 1)
         self.bn3 = FrozenBatchNorm2d(planes * 4)
         self.downsample = None
         if downsample:
             self.downsample = nn.Sequential(_conv(inplanes, planes * 4, 1, stride), FrozenBatchNorm2d(planes * 4))
         self.stride = stride
         self.dilation = dilation
+        self.groups = groups
 
 
 class ResNetBody(nn.Module):
     """Parameter tree with torchvision's names: conv1, bn1, layer1..layer4 (what IntermediateLayerGetter keeps).
     `depths` = blocks per stage (RESNET_DEPTHS); `dilate_c5` = torchvision's replace_stride_with_dilation=[False, False, True]:
-    layer4's block 0 keeps dilation 1 with stride 1 (its 1x1 downsample too), blocks 1.. are 3x3 with dilation 2 / padding 2."""
+    layer4's block 0 keeps dilation 1 with stride 1 (its 1x1 downsample too), blocks 1.. are 3x3 with dilation 2 / padding 2.
+    `groups` / `width_per_group`: torchvision's ResNeXt / wide ResNet arguments (RESNEXT_BODIES)."""
 
-    def __init__(self, depths=RESNET_DEPTHS["resnet50"], dilate_c5=False):
+    def __init__(self, depths=RESNET_DEPTHS["resnet50"], dilate_c5=False, groups=1, width_per_group=64):
         super().__init__()
         self.conv1 = nn.Conv2d(3, 64, 7, stride=2, padding=3, bias=False)
         nn.init.kaiming_normal_(self.conv1.weight, mode="fan_out", nonlinearity="relu")
@@ -89,7 +104,8 @@ class ResNetBody(nn.Module):
                     blk_stride, blk_dil = 1, (1 if i == 0 else stride)
                 else:
                     blk_stride, blk_dil = (stride if i == 0 else 1), 1
-                layers.append(Bottleneck(inplanes, planes, blk_stride, downsample=(i == 0), dilation=blk_dil))
+                layers.append(Bottleneck(inplanes, planes, blk_stride, downsample=(i == 0), dilation=blk_dil, groups=groups,
+                                         width_per_group=width_per_group))
                 inplanes = planes * 4
             setattr(self, name, nn.Sequential(*layers))
 
@@ -124,17 +140,28 @@ class _ResNetFn(Function):
         # all bottleneck weights re-laid-out to [tap][O][I] with the BN scale folded in by ONE launch per 64 tensors (52 tensors).
         # (Running this re-layout on a branch stream beside the stem was measured: 332.6 vs 332.1 img/s, within noise -- the stem
         # fills every SM, the memory-bound re-layout only finds room in its tail; not kept.)
+        # A ResNeXt's grouped conv2 weights go to the band-local layout instead, all of them by one more launch.
+        grouped = meta["grouped"]                                    # conv index -> groups
+        dense = [j for j in range(1, nconv) if j not in grouped]
         if tc.get_precision() == "bf16x3":      # (hi, lo) bf16 operands for fprop and dgrad, BN scale folded before the split
-            all_wp = [None] + tc.split_weights([w.detach() for w in weights[1:nconv]], list(scales[1:nconv]))
+            dense_wp = tc.split_weights([weights[j].detach() for j in dense], [scales[j] for j in dense])
         else:
-            all_wp = [None] + tc.pack_weights_multi(list(weights[1:nconv]), list(scales[1:nconv]))
+            dense_wp = tc.pack_weights_multi([weights[j] for j in dense], [scales[j] for j in dense])
+        all_wp = [None] * nconv
+        for j, w in zip(dense, dense_wp):
+            all_wp[j] = w
+        gj = list(grouped)
+        for j, w in zip(gj, tc.pack_grouped_multi([weights[j].detach() for j in gj], [scales[j] for j in gj],
+                                                  [grouped[j] for j in gj])):
+            all_wp[j] = w
         ci = 1
-        for bi, (stage, stride, dil, has_ds, trainable) in enumerate(meta["blocks"]):
+        for bi, (stage, stride, dil, has_ds, trainable, groups) in enumerate(meta["blocks"]):
             idx = [ci, ci + 1, ci + 2] + ([ci + 3] if has_ds else [])
             ci += len(idx)
             wp = [all_wp[j] for j in idx]
             o1 = tc.conv2d_forward(x, wp[0], shifts[idx[0]], None, 1, 1, 1, 0, relu=True, round_out=True)
-            o2 = tc.conv2d_forward(o1, wp[1], shifts[idx[1]], None, 3, 3, stride, dil, relu=True, round_out=True, dilation=dil)
+            o2 = tc.conv2d_forward(o1, wp[1], shifts[idx[1]], None, 3, 3, stride, dil, relu=True, round_out=True, dilation=dil,
+                                   groups=groups)
             if has_ds:
                 idn = tc.conv2d_forward(x, wp[3], shifts[idx[3]], None, 1, 1, stride, 0, relu=False)
             else:
@@ -170,8 +197,9 @@ class _ResNetFn(Function):
                 f += 1
         g = None                                                      # grad wrt block output, already ReLU-masked
         pending = []                                                  # 3x3 weight gradients still in packed layout
+        pending_grouped = []                                          # ... in band-local layout (grouped conv2)
         for k in range(len(blocks) - 1, -1, -1):
-            stage, stride, dil, has_ds, _ = blocks[k]
+            stage, stride, dil, has_ds, _, groups = blocks[k]
             x, o1, o2, out = ctx.saved[k]
             wp = ctx.packed[k]
             idx = conv_idx[k]
@@ -182,8 +210,9 @@ class _ResNetFn(Function):
             grads[idx[2]] = tc.conv2d_wgrad(g, o2, sc[2], 1, 1, 1, 0).view_as(_w(ctx, idx[2]))
             g2 = tc.conv2d_dgrad(g, wp[2], o2.shape, None, o2, 1, 1, 1, 0, round_out=True)
             # conv2 (3x3, maybe strided or dilated; padding = dilation)
-            pending.append((idx[1], tc.conv2d_wgrad(g2, o1, sc[1], 3, 3, stride, dil, dilation=dil)))   # [tap][O][I] -> OIHW at the end
-            g1 = tc.conv2d_dgrad(g2, wp[1], o1.shape, None, o1, 3, 3, stride, dil, round_out=True, dilation=dil)
+            dw2 = tc.conv2d_wgrad(g2, o1, sc[1], 3, 3, stride, dil, dilation=dil, groups=groups)
+            (pending if groups == 1 else pending_grouped).append((idx[1], groups, dw2))   # -> OIHW at the end
+            g1 = tc.conv2d_dgrad(g2, wp[1], o1.shape, None, o1, 3, 3, stride, dil, round_out=True, dilation=dil, groups=groups)
             # conv1
             grads[idx[0]] = tc.conv2d_wgrad(g1, x, sc[0], 1, 1, 1, 0).view_as(_w(ctx, idx[0]))
             if has_ds:
@@ -200,7 +229,10 @@ class _ResNetFn(Function):
             g = tc.conv2d_dgrad(g1, wp[0], x.shape, side, x, 1, 1, 1, 0, round_out=True)
             ctx.saved[k] = None
         ctx.saved = ctx.packed = None
-        for (j, _), dw in zip(pending, tc.unpack_wgrads_multi([d for _, d in pending], [(3, 3)] * len(pending))):
+        for (j, _, _), dw in zip(pending, tc.unpack_wgrads_multi([d for _, _, d in pending], [(3, 3)] * len(pending))):
+            grads[j] = dw
+        for (j, _, _), dw in zip(pending_grouped, tc.unpack_grouped_wgrads_multi([d for _, _, d in pending_grouped],
+                                                                                  [g for _, g, _ in pending_grouped])):
             grads[j] = dw
         return (None, None) + tuple(grads)
 
@@ -256,22 +288,31 @@ class BackboneBase(nn.Module):
             raise RuntimeError("monodetr_b200 backbone: CUDA tensors required (there is no CPU path)")
         convs = self._convs()
         sc, sh = self._bn_tensors()
-        blocks, stage_end, train_idx = [], [], []
+        blocks, stage_end, train_idx, grouped = [], [], [], {}
         ci = 1
         names = [n for n, _ in self.body.blocks()]
         for i, (name, blk) in enumerate(self.body.blocks()):
             has_ds = blk.downsample is not None
             trainable = blk.conv1.weight.requires_grad
-            blocks.append((name, blk.stride, blk.dilation, has_ds, trainable))
+            blocks.append((name, blk.stride, blk.dilation, has_ds, trainable, blk.groups))
             stage_end.append(i + 1 == len(names) or names[i + 1] != name)
             idx = [ci, ci + 1, ci + 2] + ([ci + 3] if has_ds else [])
+            if blk.groups != 1:
+                grouped[ci + 1] = blk.groups
             if trainable:
                 train_idx.append(idx)
             ci += len(idx)
-        meta = {"nconv": len(convs), "blocks": blocks, "stage_end": stage_end, "train_conv_idx": train_idx,
+        meta = {"nconv": len(convs), "blocks": blocks, "stage_end": stage_end, "train_conv_idx": train_idx, "grouped": grouped,
                 "weight_shapes": [torch.empty(c.weight.shape, device="meta") for c in convs]}
         weights = [c.weight for c in convs]
         return list(_ResNetFn.apply(images, meta, *weights, *sc, *sh))
+
+
+def _unsupported(name):
+    # resnet18 / 34 (basic blocks: the reference asserts against them) and unknown names
+    return NotImplementedError(f"monodetr_b200 backbone {name!r}: Backbone builds {', '.join(RESNET_DEPTHS)} and ResNeXtBackbone "
+                               f"builds {', '.join(RESNEXT_BODIES)}, each with dilation False or True (build_backbone picks the "
+                               "class by name)")
 
 
 class Backbone(BackboneBase):
@@ -280,11 +321,21 @@ class Backbone(BackboneBase):
 
     def __init__(self, name: str, train_backbone: bool, return_interm_layers: bool, dilation: bool):
         if name not in RESNET_DEPTHS:
-            # resnet18 / 34 (basic blocks: the reference asserts against them) and the grouped / widened convolutions of
-            # ResNeXt and wide ResNets have no kernels here
-            raise NotImplementedError(f"monodetr_b200 backbone {name!r}: supported are {', '.join(RESNET_DEPTHS)}, "
-                                      "each with dilation False or True")
+            raise _unsupported(name)
         super().__init__(ResNetBody(RESNET_DEPTHS[name], bool(dilation)), train_backbone, return_interm_layers)
+        if dilation:
+            self.strides[-1] = self.strides[-1] // 2
+
+
+class ResNeXtBackbone(BackboneBase):
+    """The same with torchvision's grouped or widened bottlenecks (RESNEXT_BODIES: resnext50_32x4d / resnext101_32x8d /
+    resnext101_64x4d, wide_resnet50_2 / wide_resnet101_2), each with or without the dilated C5 stage."""
+
+    def __init__(self, name: str, train_backbone: bool, return_interm_layers: bool, dilation: bool):
+        if name not in RESNEXT_BODIES:
+            raise _unsupported(name)
+        depths, groups, width_per_group = RESNEXT_BODIES[name]
+        super().__init__(ResNetBody(depths, bool(dilation), groups, width_per_group), train_backbone, return_interm_layers)
         if dilation:
             self.strides[-1] = self.strides[-1] // 2
 
@@ -304,5 +355,6 @@ class Joiner(nn.Sequential):
 def build_backbone(cfg):
     position_embedding = build_position_encoding(cfg)
     return_interm_layers = cfg["masks"] or cfg["num_feature_levels"] > 1
-    backbone = Backbone(cfg["backbone"], cfg["train_backbone"], return_interm_layers, cfg["dilation"])
+    cls = ResNeXtBackbone if cfg["backbone"] in RESNEXT_BODIES else Backbone
+    backbone = cls(cfg["backbone"], cfg["train_backbone"], return_interm_layers, cfg["dilation"])
     return Joiner(backbone, position_embedding)

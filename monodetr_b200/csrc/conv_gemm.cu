@@ -87,7 +87,7 @@ __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__
 // is 128 KB) the largest power of two of them that fits, reused in turn as the stores drain (see the TMA epilogue).
 template <int BN, int STAGES, int MODE, int PREC>
 struct TcSmem {
-    static constexpr bool kConvB = !(PREC == 2 && MODE == 0);
+    static constexpr bool kConvB = !(PREC == 2 && (MODE & 1) == 0);
     static constexpr int kRing = STAGES * (kTileABytes + BN * 128);
     static constexpr int kConvBuf = kConvB ? (PREC == 1 ? 2 : 1) * BN * 128 : 0;   // [hi | lo] operand tiles of one k-block
     static constexpr int kConv = 2 * kConvBuf;
@@ -96,7 +96,7 @@ struct TcSmem {
     static constexpr int kRoom = (227 * 1024 - kFixed) / (2 * 8192);   // boxes per warpgroup that fit beside the ring
     static constexpr int kBufs = kRoom >= kChunks ? kChunks : BN < 256 ? 0 : kRoom >= 4 ? 4 : kRoom >= 2 ? 2 : kRoom;
     static constexpr int kStage = 2 * kBufs * 8192;
-    static constexpr bool kTmaEpi = MODE == 0 && kBufs > 0;
+    static constexpr bool kTmaEpi = (MODE & 1) == 0 && kBufs > 0;
     static constexpr int kBytes = kFixed + (kTmaEpi ? kStage : 0);
 };
 
@@ -117,14 +117,20 @@ struct TcSmem {
 //      row per (n, k-block), written once per step by pack_gemm_weights_bf16x3.  Dropped terms are O(2^-17) per product.
 //   1  3xTF32: hi = trunc_tf32(x), lo = x - hi; the same three products as m64nBNk8 tf32 wgmma.
 //   0  single-pass TF32 (operands truncated by the tensor core; outputs optionally rounded for the next consumer).
-template <int BN, int STAGES, int MODE /*0 fprop/dgrad, 1 wgrad*/, bool B_MN, int PREC>
+// MODE 2 / 3 are the channel-banded twins of MODE 0 / 1 (grouped convolutions, see conv_grouped_check): the reduction of
+// the tile at output channel n0 covers input channels [n0, n0 + BN) only, against a band-local weight [tap][C][BN].
+// fprop / dgrad offset the A box's channel origin by n0; wgrad computes the diagonal (m0, m0) blocks only, reading the B
+// operand's channels at m0.
+template <int BN, int STAGES, int MODE /*0 fprop/dgrad, 1 wgrad, 2 / 3 banded*/, bool B_MN, int PREC>
 __global__ void __launch_bounds__(kThreadsTC, 1)
 tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                     const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapR,
                     const __grid_constant__ TcParams p) {
-    constexpr bool A_MN = (MODE == 1);
-    static_assert(!(MODE == 1) || B_MN, "wgrad reads both operands MN-major");
-    constexpr bool BF_B = (PREC == 2 && MODE == 0);               // B arrives as pre-split bf16 rows
+    constexpr bool WGRAD = (MODE & 1) != 0;
+    constexpr bool BAND = MODE >= 2;
+    constexpr bool A_MN = WGRAD;
+    static_assert(!WGRAD || B_MN, "wgrad reads both operands MN-major");
+    constexpr bool BF_B = (PREC == 2 && !WGRAD);                  // B arrives as pre-split bf16 rows
     static_assert(BN == 64 || BN == 128 || (BN == 256 && BF_B), "tile width");
     static_assert(!BF_B || !B_MN, "pre-split weights are K-major");
     constexpr bool CONVB = !BF_B;                                 // consumers rewrite B into the operand tile(s)
@@ -155,7 +161,7 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
         t.n0 = (tix % p.n_tiles_n) * BN;
         int r = tix / p.n_tiles_n;
         t.img = t.y0 = t.x0 = t.m0 = t.red_begin = t.tap = t.slice = 0;
-        if constexpr (MODE == 0) {
+        if constexpr (!WGRAD) {
             const int per_img = p.tiles_x * p.tiles_y;
             t.iters = p.ntaps * p.cblocks;
             if (p.kb_per_slice > 0) {
@@ -221,11 +227,11 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
                     uint8_t* a_dst = smem + s * kRawBytes;
                     uint8_t* b_dst = a_dst + kTileABytes;
                     mbar_arrive_expect_tx(&full_bar[s], kRawBytes);
-                    if constexpr (MODE == 0) {
+                    if constexpr (!WGRAD) {
                         const int kit = t.red_begin + it;                 // (fprop split-K: this slice's first k-block)
                         const int tap = kit / p.cblocks;
                         const int cb = kit - tap * p.cblocks;
-                        tma_load_4d(a_dst, &mapA, &full_bar[s], cb * BK, t.x0 * p.in_sx + p.tap_dx[tap],
+                        tma_load_4d(a_dst, &mapA, &full_bar[s], BAND ? t.n0 + cb * BK : cb * BK, t.x0 * p.in_sx + p.tap_dx[tap],
                                     t.y0 * p.in_sy + p.tap_dy[tap], t.img);
                         if constexpr (BF_B) {   // bf16 map: one 128-byte row = [hi 32 | lo 32] of k-block cb
                             tma_load_3d(b_dst, &mapB, &full_bar[s], cb * 64, t.n0, p.tap_w[tap]);
@@ -248,7 +254,7 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
                             tma_load_4d(a_dst + j * kChunkBytes, &mapA, &full_bar[s], t.m0 + j * 32, rx, ry, ri);
 #pragma unroll
                         for (int j = 0; j < BN / 32; ++j)
-                            tma_load_4d(b_dst + j * kChunkBytes, &mapB, &full_bar[s], t.n0 + j * 32,
+                            tma_load_4d(b_dst + j * kChunkBytes, &mapB, &full_bar[s], (BAND ? t.m0 : t.n0) + j * 32,
                                         rx * p.w_sx + (t.tap % p.wg_kw) - p.wg_pad, ry * p.w_sy + (t.tap / p.wg_kw) - p.wg_pad, ri);
                     }
                 }
@@ -542,7 +548,7 @@ tc_conv_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
             bool ok;
             size_t roff;
             float rsc = 1.f;
-            if constexpr (MODE == 0) {
+            if constexpr (!WGRAD) {
                 const int lyt = row / p.tw, lx = row - lyt * p.tw;
                 const int ib = lyt / p.th, ly = lyt - ib * p.th;  // image within the tile, row within the image
                 const int y = t.y0 + ly, x = t.x0 + lx, img = t.img + ib;
@@ -781,6 +787,20 @@ int launch_fwd(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& 
     return bn == 64 ? launch_tc<64, 6, 0, false, 0>(ma, mb, mo, mr, p, grid, stream) : launch_tc<128, 5, 0, false, 0>(ma, mb, mo, mr, p, grid, stream);
 }
 
+// Grouped convolutions (ResNeXt's 3x3 conv2: C channels in and out, `groups` groups of C / groups channels) as channel-banded
+// GEMMs.  Every group lies inside one 128-channel band when C / groups divides 128, so the 128 output channels of a tile
+// read only the 128 input channels of the same band: a tile walks taps x 4 k-blocks (MODE 2 / 3 instances) against a
+// band-local weight [tap][C][128] that is zero outside the groups.  The tensor cores do 128 / (C / groups) times the
+// grouped convolution's multiply-adds; the tile width stays 128, without the forward's split-K.
+constexpr int kBand = 128;
+
+// Launch the banded fprop / dgrad kernel (K-major band-local B operand) for the arithmetic mode.
+int launch_band(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mo, const CUtensorMap& mr, const TcParams& p, dim3 grid, int precision, cudaStream_t stream) {
+    if (precision == 2) return launch_tc<kBand, 5, 2, false, 2>(ma, mb, mo, mr, p, grid, stream);
+    if (precision == 1) return launch_tc<kBand, 3, 2, false, 1>(ma, mb, mo, mr, p, grid, stream);
+    return launch_tc<kBand, 5, 2, false, 0>(ma, mb, mo, mr, p, grid, stream);
+}
+
 struct ConvGeom {
     int B, H, W, Cin, Cout, kh, kw, stride, pad, dil, Ho, Wo;
 };
@@ -801,6 +821,17 @@ int check_geom(const ConvGeom& g, bool forward = false) {
     // TMA needs 16-byte row pitches on every operand it reads: Cin always; Cout only where dy / the output map is an
     // operand (dgrad, wgrad).  The forward epilogue writes ragged Cout with scalar stores.
     if (g.Cin % 4 || (!forward && g.Cout % 4)) return MDB_EUNSUPPORTED;
+    return 0;
+}
+
+// Geometry of a grouped (banded) convolution: 3x3, Cin == Cout == C, C % 128 == 0, C / groups dividing 128, and the dense
+// rules above (dilation > 1 only at stride 1; the weight gradient also needs pad % dilation == 0).
+int conv_grouped_check(const ConvGeom& g, int groups, bool wgrad) {
+    const int rc = check_geom(g);
+    if (rc) return rc;
+    if (groups <= 0) return MDB_EINVAL;
+    if (g.kh != 3 || g.Cin != g.Cout || g.Cin % kBand || g.Cin % groups || kBand % (g.Cin / groups)) return MDB_EUNSUPPORTED;
+    if (wgrad && g.pad % g.dil) return MDB_EUNSUPPORTED;
     return 0;
 }
 
@@ -834,9 +865,11 @@ int forward_splitk_slices(int precision, int kblocks, int bn, bool plain_epilogu
 
 // y[B,Ho,Wo,Cout] = act( conv(x[B,H,W,Cin], w) + bias + residual );  w = fp32 packed [kh*kw][Cout][Cin] (bf == false)
 // or the pre-split bf16 form [kh*kw][Cout][ceil(Cin/32)][hi 32 | lo 32] (bf == true, precision mode 2).
+// band: the grouped form (conv_grouped_check), w = band-local [kh*kw][Cout][128] (fp32) or [kh*kw][Cout][4][hi 32 | lo 32].
 int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float* bias, const float* residual, float* y,
                       int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dil, int flags,
-                      void* stream_, size_t* query_ws = nullptr /* non-null: only report the scratch bytes this call needs */) {
+                      void* stream_, size_t* query_ws = nullptr /* non-null: only report the scratch bytes this call needs */,
+                      bool band = false) {
     const int precision = bf ? 2 : (g_precision == 2 ? 1 : g_precision);   // fp32 weights in bf16x3 mode: 3xTF32
     ConvGeom g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dil);
     int rc = check_geom(g, true);
@@ -859,7 +892,7 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
     p.out_sy = p.out_sx = 1; p.out_oy = p.out_ox = 0; p.out_H = g.Ho; p.out_W = g.Wo;
     p.in_sy = p.in_sx = stride;
     p.ntaps = kh * kw;
-    p.cblocks = (Cin + BK - 1) / BK;
+    p.cblocks = band ? kBand / BK : (Cin + BK - 1) / BK;
     for (int ky = 0; ky < kh; ++ky)
         for (int kx = 0; kx < kw; ++kx) {
             const int t = ky * kw + kx;
@@ -870,7 +903,7 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
     p.bias = bias; p.residual = residual; p.relu_mask = nullptr; p.rowscale = nullptr; p.out = y;
 
     const long long out_elems = (long long)B * g.Ho * g.Wo * Cout;
-    const int slices = ((reinterpret_cast<uintptr_t>(bias) & 15u) == 0)
+    const int slices = (!band && (reinterpret_cast<uintptr_t>(bias) & 15u) == 0)
                            ? forward_splitk_slices(precision, p.ntaps * p.cblocks, Cout <= 64 ? 64 : 128, !residual && !p.relu, Cout, out_elems)
                            : 0;
     if (query_ws) {
@@ -878,7 +911,8 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
         return 0;
     }
     const int m_tiles = n_groups * p.tiles_x * p.tiles_y;
-    const int bn = precision == 2 ? pick_bn(Cout, m_tiles, slices, slices > 0 ? 32 : p.ntaps * p.cblocks) : (Cout <= 64 ? 64 : 128);
+    const int bn = band ? kBand
+                   : precision == 2 ? pick_bn(Cout, m_tiles, slices, slices > 0 ? 32 : p.ntaps * p.cblocks) : (Cout <= 64 ? 64 : 128);
     dim3 grid((Cout + bn - 1) / bn, m_tiles, 1);
 
     CUtensorMap ma, mb;
@@ -898,9 +932,10 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
         uint32_t box[3] = {64, (uint32_t)bn, 1};
         rc = make_map(&mb, w_packed, 3, dims, str, box, nullptr, true);
         if (rc) return rc;
-    } else {   // B: packed weights as (Cin, Cout, taps), box (32, BN, 1)
-        uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)Cout, (uint64_t)(kh * kw)};
-        uint64_t str[3] = {1, (uint64_t)Cin, (uint64_t)Cout * Cin};
+    } else {   // B: packed weights as (Cin, Cout, taps) (band: (128, Cout, taps)), box (32, BN, 1)
+        const uint64_t K = band ? kBand : Cin;
+        uint64_t dims[3] = {K, (uint64_t)Cout, (uint64_t)(kh * kw)};
+        uint64_t str[3] = {1, K, (uint64_t)Cout * K};
         uint32_t box[3] = {BK, (uint32_t)bn, 1};
         rc = make_map(&mb, w_packed, 3, dims, str, box, nullptr);
         if (rc) return rc;
@@ -934,14 +969,15 @@ int conv_forward_impl(const float* x, const void* w_packed, bool bf, const float
     }
     rc = setup_epi_px(p, &mo, &mr, 0, g.Wo, g.Ho, B, pix_x, pix_y, pix_b, 1);
     if (rc) return rc;
-    return launch_fwd(ma, mb, mo, mr, p, grid, bn, precision, stream);
+    return band ? launch_band(ma, mb, mo, mr, p, grid, precision, stream) : launch_fwd(ma, mb, mo, mr, p, grid, bn, precision, stream);
 }
 
 // dx[B,H,W,Cin] = (conv_transpose(dy[B,Ho,Wo,Cout], w) + residual) * (relu_mask > 0);  w = fp32 packed [taps][Cout][Cin]
 // (read MN-major) or, bf == true, the pre-split TRANSPOSED bf16 form [taps][Cin][ceil(Cout/32)][hi 32 | lo 32] (K-major).
+// band: the grouped form, w = the band-local transposed weight [taps][Cin][128] (fp32, K-major) or [taps][Cin][4][hi 32 | lo 32].
 int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float* residual, const float* relu_mask,
                     float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dil,
-                    int flags, void* stream_) {
+                    int flags, void* stream_, bool band = false) {
     const int precision = bf ? 2 : (g_precision == 2 ? 1 : g_precision);
     ConvGeom g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dil);
     int rc = check_geom(g);
@@ -971,7 +1007,7 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
             p.Ho = Hc; p.Wo = Wc;
             p.out_sy = p.out_sx = stride; p.out_oy = py; p.out_ox = px; p.out_H = H; p.out_W = W;
             p.in_sy = p.in_sx = 1;
-            p.cblocks = (Cout + BK - 1) / BK;
+            p.cblocks = band ? kBand / BK : (Cout + BK - 1) / BK;
             int nt = 0;
             for (int ky = 0; ky < kh; ++ky) {
                 if ((py + pad - ky * dil) % stride) continue;
@@ -996,13 +1032,19 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
                 rc = make_map(&ma, dy, 4, dims, str, box, nullptr);
                 if (rc) return rc;
             }
-            const int bn = bf ? pick_bn(Cin, n_groups * p.tiles_x * p.tiles_y, 0, nt * p.cblocks) : 128;
+            const int bn = band ? kBand : bf ? pick_bn(Cin, n_groups * p.tiles_x * p.tiles_y, 0, nt * p.cblocks) : 128;
             if (bf) {   // B (K-major): transposed pre-split weights as (64 * k-blocks, Cin, taps); box (64, BN, 1)
                 const uint64_t kb = (uint64_t)p.cblocks;
                 uint64_t dims[3] = {64 * kb, (uint64_t)Cin, (uint64_t)(kh * kw)};
                 uint64_t str[3] = {1, 64 * kb, (uint64_t)Cin * 64 * kb};
                 uint32_t box[3] = {64, (uint32_t)bn, 1};
                 rc = make_map(&mb, w_packed, 3, dims, str, box, nullptr, true);
+                if (rc) return rc;
+            } else if (band) {   // B (K-major): band-local transposed weights as (128, Cin, taps); box (32, BN, 1)
+                uint64_t dims[3] = {(uint64_t)kBand, (uint64_t)Cin, (uint64_t)(kh * kw)};
+                uint64_t str[3] = {1, (uint64_t)kBand, (uint64_t)Cin * kBand};
+                uint32_t box[3] = {BK, (uint32_t)kBand, 1};
+                rc = make_map(&mb, w_packed, 3, dims, str, box, nullptr);
                 if (rc) return rc;
             } else {   // B (MN-major): packed weights as (Cin, Cout, taps); box = 32 output columns (Cin) x 32 reduction rows (Cout)
                 uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)Cout, (uint64_t)(kh * kw)};
@@ -1021,7 +1063,8 @@ int conv_dgrad_impl(const float* dy, const void* w_packed, bool bf, const float*
             rc = setup_epi_px(p, &mo, &mr, (size_t)(py * W + px) * Cin, Wc, Hc, B, (uint64_t)stride * Cin,
                               (uint64_t)stride * W * Cin, (uint64_t)H * W * Cin, 1);
             if (rc) return rc;
-            if (bf) rc = launch_fwd(ma, mb, mo, mr, p, grid, bn, 2, stream);
+            if (band) rc = launch_band(ma, mb, mo, mr, p, grid, precision, stream);
+            else if (bf) rc = launch_fwd(ma, mb, mo, mr, p, grid, bn, 2, stream);
             else rc = (precision == 1) ? launch_tc<128, 3, 0, true, 1>(ma, mb, mo, mr, p, grid, stream)
                                        : launch_tc<128, 5, 0, true, 0>(ma, mb, mo, mr, p, grid, stream);
             if (rc) return rc;
@@ -1114,10 +1157,11 @@ namespace {
 
 // One weight-gradient launch of an undilated convolution between dy, a Wo x Ho pixel grid with pixel strides (dsx, dsy, dsb)
 // elements, and x, a W x H grid with pixel strides (xsx, xsy, xsb): the whole tensors, or one lattice class of a dilated
-// convolution (below).  Accumulates into dw_packed (zero-filled by the caller) with the kernel's vector reds.
+// convolution (below).  Accumulates into dw_packed (zero-filled by the caller) with the kernel's vector reds.  band: the
+// grouped form, dw_packed = the band-local [taps][Cout][128], only the diagonal (Cout tile, Cin tile) blocks computed.
 int wgrad_launch(const float* dy, const float* x, const float* rowscale, float* dw_packed, int B, int Cin, int Cout, int kh,
                  int kw, int stride, int pad, int Wo, int Ho, uint64_t dsx, uint64_t dsy, uint64_t dsb, int W, int H, uint64_t xsx,
-                 uint64_t xsy, uint64_t xsb, cudaStream_t stream) {
+                 uint64_t xsy, uint64_t xsb, cudaStream_t stream, bool band = false) {
     const int taps = kh * kw;
     TcParams p;
     memset(&p, 0, sizeof(p));
@@ -1127,7 +1171,8 @@ int wgrad_launch(const float* dy, const float* x, const float* rowscale, float* 
     p.n_img = B;
     const int total_red = B * p.rtiles_x * p.rtiles_y;
     const int bn = 128;
-    const int tiles = ((Cout + BM - 1) / BM) * ((Cin + bn - 1) / bn) * taps;
+    const int n_tiles_n = band ? 1 : (Cin + bn - 1) / bn;
+    const int tiles = ((Cout + BM - 1) / BM) * n_tiles_n * taps;
     // split-K over pixel tiles.  Large problems: ~2 waves of CTAs, but at least ~24 reduction steps per CTA so the
     // 128 x BN atomic epilogue stays a small fraction of the work.  Small problems (decoder / head linears, M = 4400 rows
     // = 138 steps): the launch is latency-bound, so spread it over up to one wave with >= 8 steps per CTA (measured
@@ -1142,7 +1187,7 @@ int wgrad_launch(const float* dy, const float* x, const float* rowscale, float* 
     splits = (total_red + p.red_per_split - 1) / p.red_per_split;
     p.w_sy = p.w_sx = stride;
     p.wg_taps = taps; p.wg_kw = kw; p.wg_pad = pad;
-    p.Mo_rows = Cout; p.No = Cin; p.ldo = Cin; p.relu = 0; p.atomic_out = 1;
+    p.Mo_rows = Cout; p.No = band ? kBand : Cin; p.ldo = p.No; p.relu = 0; p.atomic_out = 1;
     p.bias = nullptr; p.residual = nullptr; p.relu_mask = nullptr; p.rowscale = rowscale;
     p.out = dw_packed;
 
@@ -1168,25 +1213,24 @@ int wgrad_launch(const float* dy, const float* x, const float* rowscale, float* 
     CUtensorMap mo, mr;
     memset(&mo, 0, sizeof(mo));
     memset(&mr, 0, sizeof(mr));
-    dim3 grid((Cin + bn - 1) / bn, (Cout + BM - 1) / BM, taps * splits);
+    dim3 grid(n_tiles_n, (Cout + BM - 1) / BM, taps * splits);
+    if (band)
+        return g_precision == 2 ? launch_tc<kBand, 4, 3, true, 2>(ma, mb, mo, mr, p, grid, stream)
+               : g_precision == 1 ? launch_tc<kBand, 4, 3, true, 1>(ma, mb, mo, mr, p, grid, stream)
+                                  : launch_tc<kBand, 5, 3, true, 0>(ma, mb, mo, mr, p, grid, stream);
     return g_precision == 2 ? launch_tc<128, 4, 1, true, 2>(ma, mb, mo, mr, p, grid, stream)
            : g_precision == 1 ? launch_tc<128, 4, 1, true, 1>(ma, mb, mo, mr, p, grid, stream)
                               : launch_tc<128, 5, 1, true, 0>(ma, mb, mo, mr, p, grid, stream);
 }
 
-}  // namespace
-
-extern "C" {
-
-// Same with the taps `dilation` pixels apart: x[b, oy*s + ky*d - pad, ox*s + kx*d - pad, ci].  d > 1 (stride 1) also needs
-// pad % d == 0: output pixel (d*j + py, d*i + px) then reads x at (d*(j + ky - pad/d) + py, d*(i + kx - pad/d) + px), so the
-// dilated weight gradient is the sum over the d*d lattice classes (py, px) of UNDILATED ones with padding pad/d between
-// the class's pixels of dy and of x (pixel strides d).  The classes are launched one after another into the same dw (the
-// kernel adds its partial sums anyway; in reproducible mode each launch has one writer per element, in a fixed order), and
-// the kernel is the undilated one.
-int mdb_conv2d_wgrad_bias_dilated_f32(const float* dy, const float* x, const float* rowscale, float* dw_packed, float* db, int B,
-                                      int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
-                                      int accumulate, void* stream_) {
+// Weight gradient with the taps `dilation` pixels apart: x[b, oy*s + ky*d - pad, ox*s + kx*d - pad, ci].  d > 1 (stride 1)
+// also needs pad % d == 0: output pixel (d*j + py, d*i + px) then reads x at (d*(j + ky - pad/d) + py, d*(i + kx - pad/d) + px),
+// so the dilated weight gradient is the sum over the d*d lattice classes (py, px) of UNDILATED ones with padding pad/d
+// between the class's pixels of dy and of x (pixel strides d).  The classes are launched one after another into the same dw
+// (the kernel adds its partial sums anyway; in reproducible mode each launch has one writer per element, in a fixed order),
+// and the kernel is the undilated one.  band: the grouped form (dw = band-local [taps][Cout][128]).
+int wgrad_impl(const float* dy, const float* x, const float* rowscale, float* dw_packed, float* db, int B, int H, int W, int Cin,
+               int Cout, int kh, int kw, int stride, int pad, int dilation, int accumulate, void* stream_, bool band) {
     ConvGeom g = make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation);
     int rc = check_geom(g);
     if (rc) return rc;
@@ -1199,7 +1243,7 @@ int mdb_conv2d_wgrad_bias_dilated_f32(const float* dy, const float* x, const flo
     }
     const int taps = kh * kw;
     if (!accumulate) {
-        cudaError_t e = cudaMemsetAsync(dw_packed, 0, sizeof(float) * (size_t)taps * Cout * Cin, stream);
+        cudaError_t e = cudaMemsetAsync(dw_packed, 0, sizeof(float) * (size_t)taps * Cout * (band ? kBand : Cin), stream);
         if (e != cudaSuccess) return (int)e;
     }
     if (db) {
@@ -1215,9 +1259,179 @@ int mdb_conv2d_wgrad_bias_dilated_f32(const float* dy, const float* x, const flo
             rc = wgrad_launch(dy + (size_t)(py * g.Wo + px) * Cout, x + (size_t)(py * W + px) * Cin, rowscale, dw_packed, B, Cin, Cout,
                               kh, kw, stride, pad / d, Wc, Hc, (uint64_t)d * Cout, (uint64_t)d * g.Wo * Cout,
                               (uint64_t)g.Ho * g.Wo * Cout, Wx, Hx, (uint64_t)d * Cin, (uint64_t)d * W * Cin, (uint64_t)H * W * Cin,
-                              stream);
+                              stream, band);
             if (rc) return rc;
         }
+    return 0;
+}
+
+// ---- grouped weight layouts ----------------------------------------------------------------------------------------------
+// OIHW (C, C/groups, 3, 3) <-> band-local [tap][row][128]: row r's 128 k positions are the channels of r's 128-channel band,
+// zero outside r's group.  wf (forward): row = output channel, k = input channel; wd (dgrad): row = input channel, k = output
+// channel.  fp32 layout [tap][C][128]; bf16x3 layout [tap][C][4][hi 32 | lo 32] (the pre-split rows of
+// mdb_pack_gemm_weights_bf16x3).  The FrozenBN scale of the output channel is folded in before the split / rounding.
+constexpr int kMaxGrouped = 64;
+constexpr int kGroupedTaps = 9;
+struct GroupedTable {
+    const float* src[kMaxGrouped];
+    const float* scale[kMaxGrouped];
+    void* wf[kMaxGrouped];
+    void* wd[kMaxGrouped];
+    int C[kMaxGrouped], gc[kMaxGrouped];   // channels, channels per group
+};
+
+// value of band-local element (t, row, k) of wf (transposed == false) or wd (transposed == true)
+__device__ __forceinline__ float grouped_elem(const float* __restrict__ w, const float* __restrict__ scale, int gc, bool transposed,
+                                              int t, int row, int k) {
+    const int c = (row / kBand) * kBand + k;                      // the other channel: input (wf) or output (wd)
+    if (c / gc != row / gc) return 0.f;
+    const int o = transposed ? c : row, i = transposed ? row : c;
+    const float v = w[((size_t)o * gc + (i - (o / gc) * gc)) * kGroupedTaps + t];
+    return scale ? v * scale[o] : v;
+}
+
+// one thread per pair of k positions; blockIdx.y = tensor
+__global__ void pack_grouped_kernel(const __grid_constant__ GroupedTable tb, int bf, int round_tf32_out) {
+    const int j = blockIdx.y;
+    const int C = tb.C[j], gc = tb.gc[j];
+    const long long n = (long long)kGroupedTaps * C * (kBand / 2);
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int kp = (int)(i % (kBand / 2));
+        const long long r = i / (kBand / 2);
+        const int row = (int)(r % C), t = (int)(r / C);
+        for (int which = 0; which < 2; ++which) {
+            void* dst = which ? tb.wd[j] : tb.wf[j];
+            if (!dst) continue;
+            const float a = grouped_elem(tb.src[j], tb.scale[j], gc, which, t, row, 2 * kp);
+            const float b = grouped_elem(tb.src[j], tb.scale[j], gc, which, t, row, 2 * kp + 1);
+            if (bf) {   // row (t, row, k-block kp / 16): 16 words of hi, then 16 of lo
+                const uint32_t h = pack_bf16x2(a, b);
+                const uint32_t l = pack_bf16x2(a - __uint_as_float(h << 16), b - __uint_as_float(h & 0xFFFF0000u));
+                uint32_t* out = static_cast<uint32_t*>(dst) + (r * (kBand / 32) + kp / 16) * 32;
+                out[kp % 16] = h;
+                out[16 + kp % 16] = l;
+            } else {
+                float2* out = static_cast<float2*>(dst) + i;
+                *out = round_tf32_out ? make_float2(round_tf32(a), round_tf32(b)) : make_float2(a, b);
+            }
+        }
+    }
+}
+
+// dw_oihw[o][j][t] = dw_band[t][o][(o / gc) * gc + j - band(o)]: the in-group entries only
+__global__ void unpack_grouped_kernel(const __grid_constant__ GroupedTable tb) {
+    const int j = blockIdx.y;
+    const int C = tb.C[j], gc = tb.gc[j];
+    const float* __restrict__ src = tb.src[j];
+    float* __restrict__ dst = static_cast<float*>(tb.wf[j]);
+    const long long n = (long long)C * gc * kGroupedTaps;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int t = (int)(i % kGroupedTaps);
+        const long long r = i / kGroupedTaps;
+        const int ci = (int)(r % gc), o = (int)(r / gc);
+        dst[i] = src[((size_t)t * C + o) * kBand + (o / gc) * gc + ci - (o / kBand) * kBand];
+    }
+}
+
+int grouped_table(int n, int base, const float* const* src, const float* const* scale, void* const* wf, void* const* wd,
+                  const int* C, const int* groups, GroupedTable* tb, int* m) {
+    *m = n - base < kMaxGrouped ? n - base : kMaxGrouped;
+    for (int k = 0; k < *m; ++k) {
+        const int j = base + k;
+        if (!src[j] || !wf[j] || C[j] <= 0 || groups[j] <= 0) return MDB_EINVAL;
+        if (C[j] % kBand || C[j] % groups[j] || kBand % (C[j] / groups[j])) return MDB_EUNSUPPORTED;
+        tb->src[k] = src[j]; tb->scale[k] = scale ? scale[j] : nullptr;
+        tb->wf[k] = wf[j]; tb->wd[k] = wd ? wd[j] : nullptr;
+        tb->C[k] = C[j]; tb->gc[k] = C[j] / groups[j];
+    }
+    return 0;
+}
+
+int pack_grouped(int n, const float* const* w, const float* const* scale, void* const* wf, void* const* wd, const int* C,
+                 const int* groups, bool bf, void* stream) {
+    if (n < 0 || (n > 0 && (!w || !wf || !C || !groups))) return MDB_EINVAL;
+    for (int base = 0; base < n; base += kMaxGrouped) {
+        GroupedTable tb;
+        int m;
+        const int rc = grouped_table(n, base, w, scale, wf, wd, C, groups, &tb, &m);
+        if (rc) return rc;
+        pack_grouped_kernel<<<dim3(64, m), 256, 0, static_cast<cudaStream_t>(stream)>>>(tb, bf, !bf && g_precision == 0);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return (int)e;
+    }
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mdb_conv2d_wgrad_bias_dilated_f32(const float* dy, const float* x, const float* rowscale, float* dw_packed, float* db, int B,
+                                      int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                      int accumulate, void* stream_) {
+    return wgrad_impl(dy, x, rowscale, dw_packed, db, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, accumulate, stream_, false);
+}
+
+int mdb_conv2d_forward_grouped_f32(const float* x, const float* w_band, const float* bias, const float* residual, float* y, int B,
+                                   int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation, int groups,
+                                   int flags, void* stream) {
+    const int rc = conv_grouped_check(make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation), groups, false);
+    if (rc) return rc;
+    return conv_forward_impl(x, w_band, false, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags, stream,
+                             nullptr, true);
+}
+int mdb_conv2d_forward_grouped_bf16x3(const float* x, const void* w_band, const float* bias, const float* residual, float* y,
+                                      int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation,
+                                      int groups, int flags, void* stream) {
+    const int rc = conv_grouped_check(make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation), groups, false);
+    if (rc) return rc;
+    return conv_forward_impl(x, w_band, true, bias, residual, y, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags, stream,
+                             nullptr, true);
+}
+int mdb_conv2d_dgrad_grouped_f32(const float* dy, const float* w_band_t, const float* residual, const float* relu_mask, float* dx,
+                                 int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation, int groups,
+                                 int flags, void* stream) {
+    const int rc = conv_grouped_check(make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation), groups, false);
+    if (rc) return rc;
+    return conv_dgrad_impl(dy, w_band_t, false, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags,
+                           stream, true);
+}
+int mdb_conv2d_dgrad_grouped_bf16x3(const float* dy, const void* w_band_t, const float* residual, const float* relu_mask,
+                                    float* dx, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride, int pad,
+                                    int dilation, int groups, int flags, void* stream) {
+    const int rc = conv_grouped_check(make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation), groups, false);
+    if (rc) return rc;
+    return conv_dgrad_impl(dy, w_band_t, true, residual, relu_mask, dx, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, flags,
+                           stream, true);
+}
+int mdb_conv2d_wgrad_grouped_f32(const float* dy, const float* x, const float* rowscale, float* dw_band, int B, int H, int W,
+                                 int Cin, int Cout, int kh, int kw, int stride, int pad, int dilation, int groups, int accumulate,
+                                 void* stream) {
+    const int rc = conv_grouped_check(make_geom(B, H, W, Cin, Cout, kh, kw, stride, pad, dilation), groups, true);
+    if (rc) return rc;
+    return wgrad_impl(dy, x, rowscale, dw_band, nullptr, B, H, W, Cin, Cout, kh, kw, stride, pad, dilation, accumulate, stream, true);
+}
+int mdb_pack_conv_weights_grouped_multi_f32(int n, const float* const* w_oihw, const float* const* scale, float* const* wf,
+                                            float* const* wd, const int* C, const int* groups, void* stream) {
+    return pack_grouped(n, w_oihw, scale, reinterpret_cast<void* const*>(wf), reinterpret_cast<void* const*>(wd), C, groups, false,
+                        stream);
+}
+int mdb_pack_conv_weights_grouped_multi_bf16x3(int n, const float* const* w_oihw, const float* const* scale, void* const* wf,
+                                               void* const* wd, const int* C, const int* groups, void* stream) {
+    return pack_grouped(n, w_oihw, scale, wf, wd, C, groups, true, stream);
+}
+int mdb_unpack_conv_wgrads_grouped_multi_f32(int n, const float* const* dw_band, float* const* dw_oihw, const int* C,
+                                             const int* groups, void* stream) {
+    if (n < 0 || (n > 0 && (!dw_band || !dw_oihw || !C || !groups))) return MDB_EINVAL;
+    for (int base = 0; base < n; base += kMaxGrouped) {
+        GroupedTable tb;
+        int m;
+        const int rc = grouped_table(n, base, dw_band, nullptr, reinterpret_cast<void* const*>(dw_oihw), nullptr, C, groups, &tb, &m);
+        if (rc) return rc;
+        unpack_grouped_kernel<<<dim3(64, m), 256, 0, static_cast<cudaStream_t>(stream)>>>(tb);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return (int)e;
+    }
     return 0;
 }
 

@@ -175,6 +175,108 @@ def unpack_wgrad(dw_packed, kh, kw):
     return out
 
 
+# ---- grouped 3x3 convolutions (ResNeXt's conv2): band-local weights ------------------------------------------------------
+class GroupedW:
+    """A grouped 3x3 weight (C, C/groups, 3, 3) in the band-local layout of the grouped entry points (include/monodetr_b200.h,
+    "Grouped convolutions"): wf (9, C, 128) for the forward and wd (9, C, 128) for the data gradient (or None), fp32, or
+    bf16 (9, C, 4, 64) pre-split (hi, lo) rows in precision mode 'bf16x3'."""
+    __slots__ = ("wf", "wd", "C", "groups")
+
+    def __init__(self, wf, wd, C, groups):
+        self.wf, self.wd, self.C, self.groups = wf, wd, C, groups
+
+    @property
+    def split(self):
+        return self.wf.dtype == torch.bfloat16
+
+
+def pack_grouped_multi(weights, scales=None, groups=None, need_dgrad=True):
+    """[(C, C/g, 3, 3)] -> [GroupedW] in the precision mode's format, ONE launch per 64 tensors; all outputs are views of one
+    allocation.  scales[j] (C,) folds FrozenBatchNorm (backbone.py:54-64) first; groups[j] = g."""
+    n = len(weights)
+    if n == 0:
+        return []
+    scales = list(scales) if scales is not None else [None] * n
+    weights = [w if w.is_contiguous() else w.contiguous() for w in weights]
+    _chk(*weights, *[s for s in scales if s is not None])
+    split = get_precision() == "bf16x3"
+    row = 256 if split else 128                         # elements per (tap, channel) row: 4 x [hi 32 | lo 32] bf16, or 128 fp32
+    Cs = [w.shape[0] for w in weights]
+    sizes = [9 * C * row for C in Cs]
+    flat = torch.empty(((2 if need_dgrad else 1) * sum(sizes),), dtype=torch.bfloat16 if split else torch.float32,
+                       device=weights[0].device)
+    outs, wfs, wds, off = [], [], [], 0
+    for C, g, sz in zip(Cs, groups, sizes):
+        shape = (9, C, 4, 64) if split else (9, C, 128)
+        wf = flat[off:off + sz].view(shape)
+        off += sz
+        wd = flat[off:off + sz].view(shape) if need_dgrad else None
+        off += sz if need_dgrad else 0
+        outs.append(GroupedW(wf, wd, C, g))
+        wfs.append(wf)
+        wds.append(wd)
+    _lib.call("mdb_pack_conv_weights_grouped_multi_bf16x3" if split else "mdb_pack_conv_weights_grouped_multi_f32", n, weights,
+              scales, wfs, wds, _int_array(Cs), _int_array(list(groups)), launches=(n + 63) // 64)
+    return outs
+
+
+def lookup_grouped(w, groups):
+    """GroupedW of a (C, C/g, 3, 3) weight tensor: the one packed earlier in the enclosing `prepacked` context, else packed
+    now (one launch)."""
+    key = ("grouped", w.data_ptr(), tuple(w.shape), groups, get_precision())
+    if _PREPACK is not None and key in _PREPACK:
+        return _PREPACK[key]
+    gw = pack_grouped_multi([w.detach()], groups=[groups])[0]
+    if _PREPACK is not None:
+        _PREPACK[key] = gw
+    return gw
+
+
+def unpack_grouped_wgrads_multi(dw_band_list, groups_list):
+    """[(9, C, 128)] band-local weight gradients -> [(C, C/g, 3, 3)] in ONE launch per 64 tensors."""
+    n = len(dw_band_list)
+    if n == 0:
+        return []
+    _chk(*dw_band_list)
+    outs = [torch.empty((d.shape[1], d.shape[1] // g, 3, 3), dtype=torch.float32, device=d.device)
+            for d, g in zip(dw_band_list, groups_list)]
+    _lib.call("mdb_unpack_conv_wgrads_grouped_multi_f32", n, dw_band_list, outs, _int_array([d.shape[1] for d in dw_band_list]),
+              _int_array(list(groups_list)), launches=(n + 63) // 64)
+    return outs
+
+
+def _as_grouped(w, groups):
+    if isinstance(w, GroupedW):
+        assert w.groups == groups
+        return w
+    return lookup_grouped(w, groups)
+
+
+def _grouped_forward(x, w, bias, residual, stride, pad, relu, round_out, dilation, groups):
+    w = _as_grouped(w, groups)
+    _chk(x, None if w.split else w.wf, bias, residual)
+    B, H, W, C = x.shape
+    assert C == w.C
+    Ho, Wo = out_size(H, 3, stride, pad, dilation), out_size(W, 3, stride, pad, dilation)
+    y = torch.empty((B, Ho, Wo, C), dtype=torch.float32, device=x.device)
+    if residual is not None:
+        assert residual.shape == y.shape
+    _lib.call("mdb_conv2d_forward_grouped_bf16x3" if w.split else "mdb_conv2d_forward_grouped_f32", x, w.wf, bias, residual, y,
+              B, H, W, C, C, 3, 3, stride, pad, dilation, groups, int(relu) | (int(round_out) << 1))
+    return y
+
+
+def _grouped_dgrad(dy, w, x_shape, residual, relu_mask, stride, pad, round_out, dilation, groups):
+    w = _as_grouped(w, groups)
+    _chk(dy, None if w.split else w.wd, residual, relu_mask)
+    B, H, W, C = x_shape
+    assert C == w.C and dy.shape[-1] == C and w.wd is not None
+    dx = torch.empty((B, H, W, C), dtype=torch.float32, device=dy.device)
+    _lib.call("mdb_conv2d_dgrad_grouped_bf16x3" if w.split else "mdb_conv2d_dgrad_grouped_f32", dy, w.wd, residual, relu_mask, dx,
+              B, H, W, C, C, 3, 3, stride, pad, dilation, groups, int(round_out) << 1, launches=stride * stride)
+    return dx
+
+
 def colsum(x2d):
     _chk(x2d)
     M, N = x2d.shape
@@ -190,9 +292,14 @@ def _as_operand(w_packed):
     return split_weights([w_packed], packed_src=True)[0]
 
 
-def conv2d_forward(x, w_packed, bias=None, residual=None, kh=1, kw=1, stride=1, pad=0, relu=False, round_out=False, dilation=1):
+def conv2d_forward(x, w_packed, bias=None, residual=None, kh=1, kw=1, stride=1, pad=0, relu=False, round_out=False, dilation=1,
+                   groups=1):
     """w_packed: fp32 (taps, Cout, Cin) or a SplitW (precision mode 'bf16x3').  dilation > 1 (3x3, stride 1) runs the _dilated
-    entry points; dilation 1 the plain ones."""
+    entry points; dilation 1 the plain ones.  groups > 1: a grouped 3x3 through the _grouped entry points, w_packed = a GroupedW
+    or the (C, C/groups, 3, 3) weight (packed on the spot, or once per `prepacked` context)."""
+    if groups != 1:
+        assert kh == kw == 3
+        return _grouped_forward(x, w_packed, bias, residual, stride, pad, relu, round_out, dilation, groups)
     w_packed = _as_operand(w_packed)
     split = isinstance(w_packed, SplitW)
     _chk(x, None if split else w_packed, bias, residual)
@@ -223,9 +330,13 @@ def conv2d_forward(x, w_packed, bias=None, residual=None, kh=1, kw=1, stride=1, 
     return y
 
 
-def conv2d_dgrad(dy, w_packed, x_shape, residual=None, relu_mask=None, kh=1, kw=1, stride=1, pad=0, round_out=False, dilation=1):
+def conv2d_dgrad(dy, w_packed, x_shape, residual=None, relu_mask=None, kh=1, kw=1, stride=1, pad=0, round_out=False, dilation=1,
+                 groups=1):
     """w_packed: fp32 (taps, Cout, Cin) or a SplitW with .wd; dy may carry more (zero-padded) channels than a SplitW's O
-    as long as both round up to the same number of 32-wide k-blocks."""
+    as long as both round up to the same number of 32-wide k-blocks.  groups > 1: as conv2d_forward."""
+    if groups != 1:
+        assert kh == kw == 3
+        return _grouped_dgrad(dy, w_packed, x_shape, residual, relu_mask, stride, pad, round_out, dilation, groups)
     w_packed = _as_operand(w_packed)
     split = isinstance(w_packed, SplitW)
     _chk(dy, None if split else w_packed, residual, relu_mask)
@@ -248,9 +359,18 @@ def conv2d_dgrad(dy, w_packed, x_shape, residual=None, relu_mask=None, kh=1, kw=
     return dx
 
 
-def conv2d_wgrad(dy, x, rowscale=None, kh=1, kw=1, stride=1, pad=0, with_bias_grad=False, dilation=1):
+def conv2d_wgrad(dy, x, rowscale=None, kh=1, kw=1, stride=1, pad=0, with_bias_grad=False, dilation=1, groups=1):
     """dw_packed (taps, Cout, Cin); with_bias_grad=True also returns db (Cout,) = dy summed over pixels, produced by the
-    same launch (both live in one allocation so a single memset zero-fills them)."""
+    same launch (both live in one allocation so a single memset zero-fills them).  groups > 1 (a grouped 3x3, no bias): the
+    band-local (9, C, 128) gradient, for unpack_grouped_wgrads_multi."""
+    if groups != 1:
+        assert kh == kw == 3 and not with_bias_grad
+        _chk(dy, x, rowscale)
+        B, H, W, C = x.shape
+        dwb = torch.empty((9, C, 128), dtype=torch.float32, device=x.device)
+        _lib.call("mdb_conv2d_wgrad_grouped_f32", dy, x, rowscale, dwb, B, H, W, C, dy.shape[-1], 3, 3, stride, pad, dilation,
+                  groups, 0, launches=dilation * dilation)
+        return dwb
     _chk(dy, x, rowscale)
     B, H, W, Cin = x.shape
     Cout = dy.shape[-1]
