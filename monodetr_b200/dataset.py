@@ -196,9 +196,24 @@ class DeviceLoader:
         return getattr(self.loader, name)
 
     def __iter__(self):
-        for batch in self.loader:
+        return self.shard(0, 1)
+
+    def shard(self, rank, world):
+        """Batches b with b % world == rank, in order.  Every batch of the wrapped DataLoader is still drawn, so that the
+        loader's composition and order are those of the whole pass, but only this rank's batches are built on the device."""
+        for b, batch in enumerate(self.loader):
+            if b % world != rank:
+                continue
             idx = [int(k) for k, _ in batch]
             yield self.builder(self.bank.views(idx), idx, [r for _, r in batch])
+
+
+def shard_batches(loader, rank, world):
+    """Batches b with b % world == rank of `loader`, in its order: a DeviceLoader builds only those; any other iterable is run
+    whole and the other ranks' batches are dropped."""
+    if isinstance(loader, DeviceLoader):
+        return loader.shard(rank, world)
+    return (batch for b, batch in enumerate(loader) if b % world == rank)
 
 
 def check_config(cfg):

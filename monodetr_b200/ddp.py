@@ -89,6 +89,13 @@ class FlatGradBucket:
                     p.grad = v                               # the optimizer sees the reduced gradients (graph mode too)
 
 
+def rank_world():
+    """(rank, world size) of the default process group; (0, 1) without torch.distributed."""
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_rank(), dist.get_world_size()
+    return 0, 1
+
+
 def broadcast_parameters(model, src=0):
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
         for t in list(model.parameters()) + list(model.buffers()):

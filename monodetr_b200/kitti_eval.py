@@ -30,8 +30,10 @@ import re
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _lib
+from .ddp import rank_world
 
 CLASS_NAMES = ("car", "pedestrian", "cyclist", "van", "person_sitting", "truck")     # eval.py:31, lower-cased names
 CLASS_TO_NAME = {0: "Car", 1: "Pedestrian", 2: "Cyclist", 3: "Van", 4: "Person_sitting", 5: "Truck"}
@@ -448,7 +450,8 @@ class DeviceEvaluator:
       class_names  the decode class id -> name list of the tester (kitti_dataset.py:30)
 
     `add` runs extract + decode + collect (three launches on the current stream, no host synchronisation); `result` copies the
-    per-image counts to the host once, compacts the table and runs the eval; `reset` starts the next pass."""
+    per-image counts to the host once, compacts the table and runs the eval; `reset` starts the next pass; `merge` combines
+    the tables of a pass whose images were split over the ranks of a process group."""
 
     def __init__(self, gt, classes=("Car",), topk=50, threshold=0.2, cls_mean_size=None, class_names=TESTER_CLASS_NAMES,
                  image_ids=None, device=None):
@@ -482,7 +485,26 @@ class DeviceEvaluator:
         self._eval_consts = None
 
     def reset(self):
-        self.slot_info.zero_()
+        """Starts a pass.  In a single process only the per-slot counts are cleared.  With torch.distributed initialised and
+        more than one rank, the whole table is zeroed, so that the rows this rank does not add stay zero for `merge`."""
+        if rank_world()[1] > 1:
+            self._buf.zero_()
+        else:
+            self.slot_info.zero_()
+
+    def merge(self):
+        """Gives every rank the table of the whole pass, after each rank has added its own images: one all-reduce (sum) of
+        the table on the process group's backend.  Nothing happens in a single process.
+
+        The sum is exact.  `reset` zeroed every byte, and an image's rows and slot_info entries are written only by the rank
+        that added it, so when every image is added once, every byte of the table is non-zero on at most one rank.  The
+        buffer is summed as int64 words: an integer sum of words whose non-zero bytes are disjoint is their bitwise OR, with
+        no carry, so each rank's bits arrive unchanged.  A float sum would not do: it turns a -0.0 (a rounded value such as
+        -0.001) into +0.0, and the result file would print "0.00" for the reference's "-0.00".  An image added on two
+        ranks, or on none, still shows in slot_info's add count (small int32s, summed without carry), so `result()` and
+        `write_results()` raise as in a single process."""
+        if rank_world()[1] > 1:
+            dist.all_reduce(self._buf.view(torch.int64), op=dist.ReduceOp.SUM)
 
     # ------------------------------------------------------------------------------------------------------------ per batch
     def add(self, outputs, slots, img_size, calibs):

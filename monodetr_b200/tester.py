@@ -12,16 +12,34 @@ Loader contract (the reference's): batches `(inputs, calibs, targets, info)` wit
 `dataset.idx_list / label_dir / writelist / class_name / cls_mean_size`.  The batch's `calibs` (P2 of each image, as the
 val / test splits return them unchanged) feed the decode, instead of re-reading the calib files.
 `save_results(results)` is kept for callers that decode on their own.
+
+Data parallel (one process per GPU, torch.distributed initialised, W > 1 ranks): every rank runs `inference()` and
+`evaluate()`.  Rank r builds and runs batches b % W == r of the unchanged loader, so each image sees the batch it sees in a
+single process; the ranks' device tables are merged with one all-reduce (`DeviceEvaluator.merge`), rank 0 alone logs and
+writes the result files, and every rank returns the same AP.  With W = 1 nothing of this runs.
 """
 import os
 import re
 
 import torch
+import torch.distributed as dist
 
 from . import kitti_eval
+from .dataset import shard_batches
+from .ddp import rank_world
 from .trainer import load_checkpoint
 
 _EPOCH_CHECKPOINT = re.compile(r"checkpoint_epoch_(\d+)\.pth")
+
+
+class _Silent:
+    def info(self, msg):
+        pass
+
+
+def _rank0(logger):
+    """`logger` on rank 0 (and in a single process); a logger that drops every line on the other ranks."""
+    return logger if rank_world()[0] == 0 else _Silent()
 
 
 class Tester:
@@ -61,6 +79,11 @@ class Tester:
         mode = self.cfg.get("mode")
         if mode not in ("single", "all"):
             raise ValueError(f"Tester.test: cfg['mode'] must be 'single' or 'all', got {mode!r}")
+        if rank_world()[1] > 1:
+            # rank 0 may still be writing a checkpoint (Trainer.train saves checkpoint_best.pth after the last pass's
+            # result files, which the other ranks skip); every rank must load the same finished files, since their shards
+            # are merged into one table
+            dist.barrier()
         save_all = self.train_cfg["save_all"]
         if mode == "single" or not save_all:
             name = "checkpoint_epoch_{}.pth".format(self.cfg["checkpoint"]) if save_all else "checkpoint_best.pth"
@@ -80,24 +103,31 @@ class Tester:
             checkpoints = [p for _, p in sorted(found)]                # epoch order breaks ties of equal mtimes
             checkpoints.sort(key=os.path.getmtime)
         for path in checkpoints:
-            load_checkpoint(model=self.model, optimizer=None, filename=path, map_location=self.device, logger=self.logger)
+            load_checkpoint(model=self.model, optimizer=None, filename=path, map_location=self.device, logger=_rank0(self.logger))
             self.model.to(self.device)
             self.inference()
             self.evaluate()
 
     def inference(self):
+        """With torch.distributed initialised and W > 1 ranks, rank r runs batches b % W == r of the unchanged loader (the
+        single process's batches, in its order) and the ranks' tables are merged at the end; rank 0 alone logs and writes the
+        result files, and `evaluate()` returns the same AP on every rank."""
         torch.set_grad_enabled(False)
         self.model.eval()
         self.evaluator.reset()
-        for inputs, calibs, targets, info in self.dataloader:
+        rank, world = rank_world()
+        batches = self.dataloader if world == 1 else shard_batches(self.dataloader, rank, world)
+        for inputs, calibs, targets, info in batches:
             inputs = inputs.to(self.device)
             calibs = calibs.to(self.device)
             img_sizes = info["img_size"].to(self.device)
             outputs = self.model(inputs, calibs, targets, img_sizes, dn_args=0)
             slots = [self._slot[int(i)] for i in info["img_id"]]
             self.evaluator.add(outputs, slots, img_sizes, calibs)
-        self.logger.info("==> Saving ...")
-        self.evaluator.write_results(os.path.join(self.output_dir, "outputs", "data"), self.class_name)
+        self.evaluator.merge()
+        if rank == 0:
+            self.logger.info("==> Saving ...")
+            self.evaluator.write_results(os.path.join(self.output_dir, "outputs", "data"), self.class_name)
 
     def save_results(self, results):
         """The reference's save_results: {img_id: [[cls_id, alpha, x0, y0, x1, y1, h, w, l, X, Y, Z, ry, score], ...]} (what
@@ -110,5 +140,6 @@ class Tester:
                 f.write(kitti_eval.result_file_text(rows, self.class_name))
 
     def evaluate(self):
-        """Car AP3d R40 at moderate difficulty (0 when 'Car' is not in the writelist), with KITTI_Dataset.eval's log lines."""
-        return self.evaluator.result(self.logger)
+        """Car AP3d R40 at moderate difficulty (0 when 'Car' is not in the writelist), with KITTI_Dataset.eval's log lines
+        (on rank 0 only when the pass was sharded; every rank evaluates the merged table and returns the same value)."""
+        return self.evaluator.result(_rank0(self.logger))

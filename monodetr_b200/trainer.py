@@ -15,7 +15,9 @@ Two ways to run an iteration:
   (`criterion.LossLog`): the block printed every 30 batches appears as soon as its copy has arrived, at the latest at the end of
   the epoch, and no step waits for the host.  The learning rate reaches the replayed step through `optimizer.sync_hyper()`.
   With torch.distributed initialised the captured region ends after backward; the gradient all-reduce and the optimizer's two
-  launches follow it, parameters are broadcast from rank 0 at construction and only rank 0 prints, logs and saves.
+  launches follow it, parameters are broadcast from rank 0 at construction and only rank 0 prints, logs and saves.  With
+  this package's `Tester` attached, every rank runs its `inference()` / `evaluate()` (it splits the pass over the ranks) and
+  so keeps the same `best_result` / `best_epoch`; any other tester runs on rank 0 alone.
 * Eager path -- anything else (the reference's own criterion, a torch optimizer): the reference's loop as it is written, with
   `prepare_targets` and the `.item()` log.
 
@@ -179,6 +181,10 @@ class Trainer(object):
     def live_graphs(self):
         return sum(1 for s in self._steps.values() if s.graph is not None)
 
+    def _tester_splits(self):
+        from .tester import Tester                # tester imports this module
+        return isinstance(self.tester, Tester)
+
     def train(self):
         start_epoch = self.epoch
 
@@ -201,26 +207,31 @@ class Trainer(object):
             if hasattr(self.optimizer, "sync_hyper"):
                 self.optimizer.sync_hyper()           # the new lr reaches the device block a replayed step reads
 
-            # save trained model
-            if (self.epoch % self.cfg["save_frequency"]) == 0 and self.is_main:
-                os.makedirs(self.output_dir, exist_ok=True)
-                if self.cfg["save_all"]:
-                    ckpt_name = os.path.join(self.output_dir, "checkpoint_epoch_%d" % self.epoch)
-                else:
-                    ckpt_name = os.path.join(self.output_dir, "checkpoint")
+            # save trained model; rank 0 saves and logs.  This package's Tester splits its pass over the ranks, so every rank
+            # runs it; any other tester (the reference's, which does not split) runs on rank 0 alone, as in the reference
+            if (self.epoch % self.cfg["save_frequency"]) == 0:
+                if self.is_main:
+                    os.makedirs(self.output_dir, exist_ok=True)
+                    if self.cfg["save_all"]:
+                        ckpt_name = os.path.join(self.output_dir, "checkpoint_epoch_%d" % self.epoch)
+                    else:
+                        ckpt_name = os.path.join(self.output_dir, "checkpoint")
 
-                save_checkpoint(get_checkpoint_state(self.model, self.optimizer, self.epoch, best_result, best_epoch), ckpt_name)
+                    save_checkpoint(get_checkpoint_state(self.model, self.optimizer, self.epoch, best_result, best_epoch), ckpt_name)
 
-                if self.tester is not None:
-                    self.logger.info("Test Epoch {}".format(self.epoch))
+                if self.tester is not None and (self.is_main or self._tester_splits()):
+                    if self.is_main:
+                        self.logger.info("Test Epoch {}".format(self.epoch))
                     self.tester.inference()
                     cur_result = self.tester.evaluate()
                     if cur_result > best_result:
                         best_result = cur_result
                         best_epoch = self.epoch
-                        ckpt_name = os.path.join(self.output_dir, "checkpoint_best")
-                        save_checkpoint(get_checkpoint_state(self.model, self.optimizer, self.epoch, best_result, best_epoch), ckpt_name)
-                    self.logger.info("Best Result:{}, epoch:{}".format(best_result, best_epoch))
+                        if self.is_main:
+                            ckpt_name = os.path.join(self.output_dir, "checkpoint_best")
+                            save_checkpoint(get_checkpoint_state(self.model, self.optimizer, self.epoch, best_result, best_epoch), ckpt_name)
+                    if self.is_main:
+                        self.logger.info("Best Result:{}, epoch:{}".format(best_result, best_epoch))
 
             progress_bar.update()
 
