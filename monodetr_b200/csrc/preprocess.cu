@@ -5,8 +5,11 @@
 // produces the normalised NCHW fp32 batch the backbone reads: optional left-right flip (:140-142), inverse affine map of every
 // output pixel centre, PIL's bilinear filter (clamped neighbours, zero fill outside, result truncated to 8 bits), /255,
 // (x - mean) / std (:159-161).
-// Arithmetic: coordinates and interpolation in fp64 exactly as PIL's C code (Geometry.c) so that the 8-bit value is
-// bit-identical; the float conversion in fp32 exactly as numpy's.  HBM-bound: 12 bytes written per output pixel.
+// Arithmetic: coordinates and interpolation in fp64 in the order and with the roundings of PIL's C code (Geometry.c, built
+// without FMA): xin = (a0*xc + a1*yc) + a2, then - 0.5, and v = a + (b - a) * d, every product rounded before its sum by an
+// explicit _rn intrinsic, so that the floor of each coordinate and the 8-bit truncation are bit-identical to Pillow's for any
+// affine map, sheared or not (tests/test_preprocess_edges_gpu.py); the float conversion in fp32 exactly as numpy's.
+// HBM-bound: 12 bytes written per output pixel.
 // Before it, when the dataset's `aug_pd` is on, a second kernel applies the reference's photometric distortion (:136-138,
 // pd.py:376-397) to every source image with its own host-drawn parameters and writes the 8-bit result to a caller buffer that the
 // warp then reads: pointwise, 3 bytes read and 3 written per source pixel.
@@ -20,6 +23,9 @@
 
 namespace {
 
+// Pillow's BILINEAR(v, a, b, d): a + (b - a) * d with the product rounded before the sum (nvcc would otherwise fuse it to a DFMA)
+__device__ __forceinline__ double lerp_rn(double a, double b, double d) { return __dadd_rn(a, __dmul_rn(__dsub_rn(b, a), d)); }
+
 __global__ void __launch_bounds__(256) warp_affine_normalize_kernel(const unsigned char* const* __restrict__ src, const int* __restrict__ src_wh,
                                                                     const long long* __restrict__ src_pitch, const double* __restrict__ trans_inv,
                                                                     const unsigned char* __restrict__ flip, float* __restrict__ out, int Wo,
@@ -30,13 +36,13 @@ __global__ void __launch_bounds__(256) warp_affine_normalize_kernel(const unsign
     const int W = src_wh[2 * b], H = src_wh[2 * b + 1];
     const double* a = trans_inv + 6 * b;
     const double xc = x + 0.5, yc = y + 0.5;
-    double xin = a[0] * xc + a[1] * yc + a[2];
-    double yin = a[3] * xc + a[4] * yc + a[5];
+    double xin = __dadd_rn(__dadd_rn(__dmul_rn(a[0], xc), __dmul_rn(a[1], yc)), a[2]);
+    double yin = __dadd_rn(__dadd_rn(__dmul_rn(a[3], xc), __dmul_rn(a[4], yc)), a[5]);
     float v[3] = {0.f, 0.f, 0.f};
     if (!(xin < 0.0 || xin >= (double)W || yin < 0.0 || yin >= (double)H)) {
-        xin -= 0.5; yin -= 0.5;
+        xin = __dsub_rn(xin, 0.5); yin = __dsub_rn(yin, 0.5);
         const int xf = (int)floor(xin), yf = (int)floor(yin);
-        const double dx = xin - xf, dy = yin - yf;
+        const double dx = __dsub_rn(xin, xf), dy = __dsub_rn(yin, yf);
         int x0 = min(max(xf, 0), W - 1), x1 = min(max(xf + 1, 0), W - 1);
         const int y0 = min(max(yf, 0), H - 1);
         const bool has_y1 = yf + 1 >= 0 && yf + 1 < H;
@@ -46,13 +52,13 @@ __global__ void __launch_bounds__(256) warp_affine_normalize_kernel(const unsign
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
             const double p00 = r0[x0 * 3 + c], p01 = r0[x1 * 3 + c];
-            const double v1 = p00 + (p01 - p00) * dx;
+            const double v1 = lerp_rn(p00, p01, dx);
             double v2 = v1;
             if (has_y1) {
                 const double p10 = r1[x0 * 3 + c], p11 = r1[x1 * 3 + c];
-                v2 = p10 + (p11 - p10) * dx;
+                v2 = lerp_rn(p10, p11, dx);
             }
-            v[c] = (float)(unsigned char)(v1 + (v2 - v1) * dy);
+            v[c] = (float)(unsigned char)lerp_rn(v1, v2, dy);
         }
     }
     const size_t plane = (size_t)Ho * Wo;

@@ -131,6 +131,33 @@ def distort_float(img_u8, p: Params, simd_width=SIMD_WIDTH):
     return x[..., list(PERMS[p.perm])]
 
 
+def distort_float_rows(img_u8, p: Params, simd_width=SIMD_WIDTH, workers=8):
+    """distort_float over blocks of rows on a thread pool (numpy releases the GIL in its loops): the same bits, since each row
+    is converted on its own.  For the all-colour images, where one call is 2**24 pixels."""
+    from concurrent.futures import ThreadPoolExecutor
+    blocks = np.array_split(np.arange(img_u8.shape[0]), workers)
+    with ThreadPoolExecutor(workers) as ex:
+        parts = ex.map(lambda r: distort_float(img_u8[r[0]:r[-1] + 1], p, simd_width), [r for r in blocks if len(r)])
+        return np.concatenate(list(parts))
+
+
+def every_colour(W):
+    """All 2**24 8-bit colours, in order, in one (ceil(2**24 / W), W, 3) image; a last partial row is filled with colour 0.
+    W % SIMD_WIDTH == 0 sends every pixel through cv2's vector loop, W < SIMD_WIDTH through its scalar loop."""
+    n = 1 << 24
+    H = -(-n // W)
+    c = np.zeros(H * W, np.uint32)
+    c[:n] = np.arange(n, dtype=np.uint32)
+    return np.stack([c >> 16, (c >> 8) & 255, c & 255], -1).astype(np.uint8).reshape(H, W, 3)
+
+
+# Records at the ends of the sampled ranges (brightness +-32, contrast and saturation 0.5 / 1.5, hue +-18), both contrast orders,
+# every channel permutation, and the neutral record.
+EDGE_RECORDS = (Params(32.0, 1.5, 1.5, 18.0, 0, 0), Params(-32.0, 0.5, 0.5, -18.0, 1, 1), Params(32.0, 0.5, 1.5, -18.0, 0, 2),
+                Params(-32.0, 1.5, 0.5, 18.0, 1, 3), Params(0.0, 1.5, 1.5, 18.0, 1, 4), Params(32.0, 1.5, 0.5, -18.0, 1, 5),
+                Params(-32.0, 0.5, 1.5, 18.0, 0, 5), Params())
+
+
 def to_u8(x):
     """numpy's float32 -> uint8 cast as it behaves on x86: truncate toward zero, keep the low 8 bits."""
     return np.trunc(x).astype(np.int64).astype(np.uint8)

@@ -7,7 +7,9 @@
   flip                   kitti_dataset.py:140-142   Image.FLIP_LEFT_RIGHT
 
 Pinned against Pillow itself and the reference's get_affine_transform (cv2) by tests/golden/preprocess.npz
-(tools/gen_golden_preprocess.py) -- tests/test_oracle_preprocess.py.
+(tools/gen_golden_preprocess.py) -- tests/test_oracle_preprocess.py; and against live Pillow on inputs constructed to sit on a
+coordinate floor or an 8-bit truncation edge (tests/golden/preprocess_edges.npz) -- tests/test_preprocess_edges_host_logic.py.
+numpy rounds every product before its sum, as Pillow's C code does.
 """
 import numpy as np
 
