@@ -13,6 +13,7 @@ Execution is ONE hand-scheduled autograd Function (no cuDNN, no per-layer autogr
   * backward: dgrad kernels apply the previous ReLU's mask (and add the identity-branch gradient) in their
     epilogue, wgrad kernels multiply by the BN scale per output row; layer1 and the stem get no backward.
 """
+import os
 from typing import List
 
 import torch
@@ -34,6 +35,18 @@ RESNEXT_BODIES = {
     "resnext101_64x4d": (RESNET_DEPTHS["resnet101"], 64, 4),
     "wide_resnet50_2": (RESNET_DEPTHS["resnet50"], 1, 128),
     "wide_resnet101_2": (RESNET_DEPTHS["resnet101"], 1, 128),
+}
+# torchvision's IMAGENET1K_V1 checkpoint of each body, which the reference's `pretrained=True` loads: (file name under
+# torch.hub.get_dir()/checkpoints, torchvision weights enum).  A dilated C5 stage has the same weights.
+IMAGENET1K_V1 = {
+    "resnet50": ("resnet50-0676ba61.pth", "ResNet50_Weights"),
+    "resnet101": ("resnet101-63fe2227.pth", "ResNet101_Weights"),
+    "resnet152": ("resnet152-394f9c45.pth", "ResNet152_Weights"),
+    "resnext50_32x4d": ("resnext50_32x4d-7cdf4587.pth", "ResNeXt50_32X4D_Weights"),
+    "resnext101_32x8d": ("resnext101_32x8d-8ba56ff5.pth", "ResNeXt101_32X8D_Weights"),
+    "resnext101_64x4d": ("resnext101_64x4d-173b62eb.pth", "ResNeXt101_64X4D_Weights"),
+    "wide_resnet50_2": ("wide_resnet50_2-95faca4d.pth", "Wide_ResNet50_2_Weights"),
+    "wide_resnet101_2": ("wide_resnet101_2-32ee1156.pth", "Wide_ResNet101_2_Weights"),
 }
 
 
@@ -352,9 +365,62 @@ class Joiner(nn.Sequential):
         return feats, pos
 
 
+def imagenet_checkpoint_path(name):
+    """Where torchvision keeps the IMAGENET1K_V1 file of backbone `name`: torch.hub.get_dir()/checkpoints/<file>."""
+    return os.path.join(torch.hub.get_dir(), "checkpoints", IMAGENET1K_V1[name][0])
+
+
+def load_imagenet_weights(body, name, source=True):
+    """Copy a torchvision ImageNet state_dict into `body` (a ResNetBody built for backbone `name`), bit for bit.
+
+    source: True reads torchvision's IMAGENET1K_V1 file from the torch hub cache (imagenet_checkpoint_path), a path reads that
+    file.  Nothing is downloaded: a missing file raises FileNotFoundError.  `fc.*` and `num_batches_tracked` entries are
+    ignored; every other entry must be one of the body's, with its shape and finite values, and every body entry must be
+    present (ValueError names the first that is not).  Draws no random numbers, and may run on a body that has already run
+    a forward: the folded BN tensors and weight splits are rebuilt from the new values."""
+    if source is True:
+        path = imagenet_checkpoint_path(name)
+        if not os.path.isfile(path):
+            raise FileNotFoundError(f"backbone {name!r}: torchvision's ImageNet weights ({IMAGENET1K_V1[name][1]}.IMAGENET1K_V1) "
+                                    f"are not at {path}; place the file there (or give its path as pretrained_backbone)")
+    else:
+        path = os.fspath(source)
+        if not os.path.isfile(path):
+            raise FileNotFoundError(f"backbone {name!r}: no ImageNet weights file at {path}")
+    sd = torch.load(path, map_location="cpu", weights_only=True)
+    sd = {k: v for k, v in sd.items() if not k.startswith("fc.") and not k.endswith("num_batches_tracked")}
+    own = body.state_dict()
+    for k, t in own.items():
+        if k not in sd:
+            raise ValueError(f"{path}: no entry {k!r} of backbone {name!r}")
+        v = sd[k]
+        if tuple(v.shape) != tuple(t.shape):
+            raise ValueError(f"{path}: {k!r} has shape {tuple(v.shape)}, backbone {name!r} needs {tuple(t.shape)}")
+        if not v.is_floating_point() or not bool(torch.isfinite(v).all()):
+            raise ValueError(f"{path}: {k!r} holds non-finite or non-floating-point values")
+    for k in sd:
+        if k not in own:
+            raise ValueError(f"{path}: entry {k!r} is not part of backbone {name!r}")
+    with torch.no_grad():
+        for k, t in own.items():
+            t.copy_(sd[k])
+
+
 def build_backbone(cfg):
+    """cfg["pretrained_backbone"] (default False: random initialisation): True or a file path loads torchvision's ImageNet
+    weights into the ResNet body (load_imagenet_weights) on the main process only -- rank 0 of an initialised default process
+    group, like the reference's `pretrained=is_main_process()`.  The other ranks keep their random weights: `Trainer`
+    broadcasts rank 0's parameters and buffers when it is constructed; other callers must broadcast them themselves."""
     position_embedding = build_position_encoding(cfg)
     return_interm_layers = cfg["masks"] or cfg["num_feature_levels"] > 1
     cls = ResNeXtBackbone if cfg["backbone"] in RESNEXT_BODIES else Backbone
     backbone = cls(cfg["backbone"], cfg["train_backbone"], return_interm_layers, cfg["dilation"])
+    pretrained = cfg.get("pretrained_backbone", False)
+    if pretrained is not False and pretrained is not None and _is_main_process():
+        load_imagenet_weights(backbone.body, cfg["backbone"], pretrained)
     return Joiner(backbone, position_embedding)
+
+
+def _is_main_process():
+    import torch.distributed as dist
+    return not (dist.is_available() and dist.is_initialized()) or dist.get_rank() == 0
