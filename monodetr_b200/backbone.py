@@ -272,6 +272,9 @@ class BackboneBase(nn.Module):
         self._bn_cache = None
 
     def _bn_tensors(self):
+        """The frozen BatchNorms folded into per-channel scale / shift, recomputed when a buffer has changed.  On the same
+        device the new values are written into the tensors already handed out, so that a CUDA graph captured with them (the
+        Detector's) reads the buffers as they are after a load_state_dict."""
         key = tuple(b._version for b in self.body.buffers()) + (str(next(self.body.buffers()).device),)
         if self._bn_cache is None or self._bn_cache[0] != key:
             sc, sh = [], []
@@ -280,6 +283,11 @@ class BackboneBase(nn.Module):
                     a, b = bn.scale_shift()
                     sc.append(a)
                     sh.append(b)
+                old = self._bn_cache
+                if old is not None and old[0][-1] == key[-1]:
+                    for dst, src in zip(old[1] + old[2], sc + sh):
+                        dst.copy_(src)
+                    sc, sh = old[1], old[2]
             self._bn_cache = (key, sc, sh)
         return self._bn_cache[1], self._bn_cache[2]
 

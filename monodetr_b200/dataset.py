@@ -49,15 +49,22 @@ def read_image_sizes(paths):
     sizes = np.zeros((len(paths), 2), np.int64)
     for i, p in enumerate(paths):
         with Image.open(p) as im:
-            if im.mode != "RGB":
-                raise ValueError(f"{p}: mode {im.mode!r}; only 8-bit RGB images are supported")
+            _check_rgb(p, im)
             sizes[i] = im.size
     return sizes
 
 
-def _decode(path):
+def _check_rgb(path, im):
+    if im.mode != "RGB":
+        raise ValueError(f"{path}: mode {im.mode!r}; only 8-bit RGB images are supported")
+
+
+def decode_image(path):
+    """The (H, W, 3) uint8 array of an 8-bit RGB image file, as the reference reads it (np.array of the Pillow image);
+    ValueError naming the file for any other mode."""
     from PIL import Image
     with Image.open(path) as im:
+        _check_rgb(path, im)
         return np.array(im)
 
 
@@ -79,7 +86,7 @@ class ImageBank:
             raise RuntimeError("ImageBank: a CUDA device is required")
         self.data = torch.empty(max(int(self.offsets[-1]), 1), dtype=torch.uint8, device=self.device)
         with ThreadPoolExecutor(max(1, int(threads))) as pool:      # PIL releases the GIL while it inflates
-            for k, arr in enumerate(pool.map(_decode, paths)):
+            for k, arr in enumerate(pool.map(decode_image, paths)):
                 W, H = (int(v) for v in self.sizes[k])
                 if arr.shape != (H, W, 3) or arr.dtype != np.uint8:
                     raise ValueError(f"{paths[k]}: decoded to {arr.shape} {arr.dtype}, header said ({H}, {W}, 3) uint8")

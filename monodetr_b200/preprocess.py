@@ -7,6 +7,9 @@
   PhotometricDistort().sample()                                       lib/datasets/kitti/pd.py:376-397 (`aug_pd`): the host draws
   ImageBatchPreprocessor(...)(images_u8, trans_inv, flip, distort=[records])  the distortion on the device first (a second launch,
                                                                       csrc/preprocess.cu), bit-identical to pd.py + cv2 + numpy
+  ImageBatchPreprocessor(...).metadata(buf, ...) + .launch(meta, B, out)   the same call in two steps: host metadata into a
+                                                                      caller's buffer, then the launch from its device copy
+                                                                      (what a captured CUDA graph replays)
 
 `images_u8`: list of (H_i, W_i, 3) uint8 tensors (ragged, as decoded; CPU tensors are uploaded through pinned memory, CUDA tensors
 are used in place).  The result is bit-identical to PIL's AFFINE/BILINEAR transform followed by the reference's numpy
@@ -160,6 +163,11 @@ def pack_photometric(records, B):
     return out
 
 
+def metadata_words(B, distort=False):
+    """Length in int64 words of the metadata ImageBatchPreprocessor.metadata writes for B images."""
+    return B * 9 + (B + 7) // 8 + (5 * B if distort else 0)
+
+
 def _require_cuda(device):
     if device.type != "cuda":
         raise RuntimeError("ImageBatchPreprocessor: a CUDA device is required (there is no CPU path)")
@@ -175,38 +183,62 @@ class ImageBatchPreprocessor:
     def __call__(self, images, trans_inv, flip=None, distort=None):
         """images: list of (H, W, 3) uint8 tensors; trans_inv: (B, 2, 3) array (PIL `data`); flip: optional (B,) bools;
         distort: optional list of B PhotometricParams (PhotometricDistort.sample()), applied to each source image before the flip
-        and the warp, as the reference's `aug_pd`.  The images themselves are never modified."""
+        and the warp, as the reference's `aug_pd`.  The images themselves are never modified.
+
+        Two steps, which a caller that replays the launch as a CUDA graph takes one by one: `metadata` fills a host buffer,
+        ONE pinned upload puts it on the device, and `launch` runs the kernels from there."""
         B = len(images)
         _require_cuda(self.device)
         records = None if distort is None else pack_photometric(distort, B)
         dev_imgs = self._device_images(images)
-        # ONE pinned upload for all per-image metadata: pointers | pitches | matrices (fp64) | (W, H) int32 pairs | flip flags
-        # [| distorted-image pointers | their pitches | distortion records]
-        n_base = B * 9 + (B + 7) // 8
-        buf = np.zeros(n_base + (0 if records is None else 5 * B), np.int64)
-        for i, im in enumerate(dev_imgs):
-            buf[i], buf[B + i] = im.data_ptr(), im.stride(0)
-        buf[2 * B:8 * B].view(np.float64)[:] = np.asarray(trans_inv, np.float64).reshape(B * 6)
-        wh = buf[8 * B:9 * B].view(np.int32)
-        wh[0::2], wh[1::2] = [im.shape[1] for im in dev_imgs], [im.shape[0] for im in dev_imgs]
-        if flip is not None:
-            buf[9 * B:n_base].view(np.uint8)[:B] = np.asarray(flip).astype(np.uint8)
-        scratch = None
+        distorted, scratch = None, None
         if records is not None:
             # one flat buffer holds every distorted image, rows packed (pitch 3 * W)
             sizes = [im.shape[0] * im.shape[1] * 3 for im in dev_imgs]
             scratch = torch.empty(max(sum(sizes), 1), dtype=torch.uint8, device=self.device)
-            offs = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64)
-            buf[n_base:n_base + B] = scratch.data_ptr() + offs
-            buf[n_base + B:n_base + 2 * B] = [3 * im.shape[1] for im in dev_imgs]
-            buf[n_base + 2 * B:n_base + 5 * B].view(_RECORD_DTYPE)[:] = records
+            distorted = scratch.data_ptr() + np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64)
+        buf = np.empty(metadata_words(B, records is not None), np.int64)
+        self.metadata(buf, [im.data_ptr() for im in dev_imgs], [im.stride(0) for im in dev_imgs],
+                      [(im.shape[1], im.shape[0]) for im in dev_imgs], trans_inv, flip, distorted, records)
         meta = torch.from_numpy(buf).pin_memory().to(self.device, non_blocking=True)
-        base = meta.data_ptr()
-        ptrs, pitch, trd, whd, fld = base, base + 8 * B, base + 16 * B, base + 64 * B, base + 72 * B
         W, H = self.resolution
         out = torch.empty(B, 3, H, W, dtype=torch.float32, device=self.device)
+        return self.launch(meta.data_ptr(), B, out, distort=records is not None)
+
+    @staticmethod
+    def metadata(buf, ptrs, pitches, sizes, trans_inv, flip=None, distorted=None, records=None):
+        """Writes the per-image metadata of B images into `buf`, an int64 host array of at least
+        `metadata_words(B, records is not None)` words (the rest is left alone): source pointers | row pitches in bytes |
+        trans_inv matrices (fp64) | (W, H) int32 pairs | flip flags [| `distorted` -- where the distortion writes each image,
+        rows packed -- | their pitches | distortion records (pack_photometric)].  `sizes` is (B, 2) [W, H].  Returns `buf`."""
+        B = len(ptrs)
+        n_base = B * 9 + (B + 7) // 8
+        buf[:metadata_words(B, records is not None)] = 0
+        buf[:B], buf[B:2 * B] = ptrs, pitches
+        buf[2 * B:8 * B].view(np.float64)[:] = np.asarray(trans_inv, np.float64).reshape(B * 6)
+        wh = buf[8 * B:9 * B].view(np.int32)
+        sizes = np.asarray(sizes, np.int64).reshape(B, 2)
+        wh[0::2], wh[1::2] = sizes[:, 0], sizes[:, 1]
+        if flip is not None:
+            buf[9 * B:n_base].view(np.uint8)[:B] = np.asarray(flip).astype(np.uint8)
+        if records is not None:
+            buf[n_base:n_base + B] = distorted
+            buf[n_base + B:n_base + 2 * B] = 3 * sizes[:, 0]
+            buf[n_base + 2 * B:n_base + 5 * B].view(_RECORD_DTYPE)[:] = records
+        return buf
+
+    def launch(self, meta, B, out, distort=False):
+        """Runs the distortion (with `distort`) and the warp of B images on the current stream, reading the metadata that
+        `metadata` laid out at device address `meta`, into `out` ((B, 3, H, W) float32 CUDA tensor at this resolution).  Reads
+        nothing from the host but the mean and std, so a CUDA graph can capture it.  Returns `out`."""
+        W, H = self.resolution
+        if out.shape != (B, 3, H, W) or out.dtype != torch.float32 or not out.is_contiguous():
+            raise ValueError(f"ImageBatchPreprocessor.launch: out must be a contiguous ({B}, 3, {H}, {W}) float32 tensor")
+        n_base = B * 9 + (B + 7) // 8
+        base = int(meta)
+        ptrs, pitch, trd, whd, fld = base, base + 8 * B, base + 16 * B, base + 64 * B, base + 72 * B
         with torch.cuda.device(self.device):
-            if records is not None:
+            if distort:
                 dptrs, dpitch, recd = base + 8 * n_base, base + 8 * (n_base + B), base + 8 * (n_base + 2 * B)
                 _lib.call("mdb_photometric_distort_u8", ptrs, whd, pitch, recd, dptrs, dpitch, B)
                 ptrs, pitch = dptrs, dpitch                     # the warp samples the distorted images
