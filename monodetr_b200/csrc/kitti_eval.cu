@@ -12,7 +12,8 @@
 // fp32, with explicit _rn intrinsics wherever nvcc could contract a multiply and an add into an FMA (the reference's loops are plain
 // IEEE operations, so a contraction would flip `overlap > min_overlap` decisions).  Counts are integers (atomics are exact in any
 // order); the AOS similarity is summed in gt order per image and then in image order, so the result does not depend on scheduling.
-// Parity: tests/test_kitti_eval_gpu.py against oracle/kitti_eval.py and the golden vectors generated from the reference.
+// Parity: tests/test_kitti_eval_gpu.py against oracle/kitti_eval.py and the golden vectors generated from the reference;
+// tests/test_kitti_eval_edges_gpu.py bit for bit where overlaps sit exactly at, or one or two ulps around, the thresholds.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>

@@ -79,6 +79,11 @@ def _segment(p1, p2, i, j):
     return (ABBA * DC0 - BA0 * CDDC) / DH, (ABBA * DC1 - BA1 * CDDC) / DH
 
 
+def _triangle_area(a, b, c):
+    """rotate_iou.py:17-20: signed area of the triangle (a, b, c)."""
+    return ((a[0] - c[0]) * (b[1] - c[1]) - (a[1] - c[1]) * (b[0] - c[0])) / F32(2)
+
+
 def rotated_intersection(rb1, rb2):
     """rotate_iou.py:231-245: area of the intersection of two rotated boxes, fp32 (rb = [x, y, dx, dy, angle] float32)."""
     c1, c2 = _corners(rb1), _corners(rb2)
@@ -93,6 +98,10 @@ def rotated_intersection(rb1, rb2):
             t = _segment(c1, c2, i, j)
             if t is not None:
                 pts.append(list(t))
+    # The reference's int_pts holds 8 points.  A degenerate pair can give more (the same box with its heading flipped between
+    # float32(pi / 2) and float32(-pi / 2)): the reference's simulator run raises there and its GPU run writes past a local
+    # array.  Here, as in csrc/kitti_eval.cu, the first 8 candidates in the reference's order are kept.
+    pts = pts[:8]
     n = len(pts)
     if n > 0:                                                        # rotate_iou.py:33-70 (insertion sort by pseudo-angle)
         cx, cy = F32(0), F32(0)
@@ -118,8 +127,7 @@ def rotated_intersection(rb1, rb2):
                 vs[j], pts[j] = tmp, tp
     area = F32(0)                                                    # rotate_iou.py:17-30
     for i in range(n - 2):
-        a, b, c = pts[0], pts[i + 1], pts[i + 2]
-        area = area + abs(((a[0] - c[0]) * (b[1] - c[1]) - (a[1] - c[1]) * (b[0] - c[0])) / F32(2))
+        area = area + abs(_triangle_area(pts[0], pts[i + 1], pts[i + 2]))
     return area
 
 

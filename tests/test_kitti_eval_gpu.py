@@ -63,17 +63,11 @@ def random_set(rng, n_img, max_gt=8, max_dt=12):
 def test_overlaps_match_reference(golden, case):
     gt, dt = annos(golden, case)
     blocks = ke.image_overlaps(gt, dt)
-    worst = []
     for m in range(3):
         got = np.concatenate([b.reshape(-1) for b in blocks[m]])
         ref = golden[f"{case}__ov{m}"]
         assert got.shape == ref.shape
-        if m == 0:
-            np.testing.assert_array_equal(got, ref)
-        elif ref.size:
-            worst.append(float(np.abs(got - ref).max()))
-            assert worst[-1] <= 1e-6
-    print(f"case {case}: max |BEV, 3d overlap - reference| = {worst}")
+        np.testing.assert_array_equal(got, ref)                 # BEV / 3d: the reference's fp32 arithmetic, bit for bit
 
 
 @pytest.mark.parametrize("case", CASES)
@@ -114,15 +108,10 @@ def test_random_set_matches_oracle():
     gt, dt = [gt[b] for b in keep], [dt[b] for b in keep]
     assert len(gt) > 250
     blocks = ke.image_overlaps(gt, dt)
-    worst = 0.0
     for b, (g, d) in enumerate(zip(gt, dt)):
         ref = ok.image_overlaps(g, d)
-        np.testing.assert_array_equal(blocks[0][b], ref[0])
-        for m in (1, 2):
-            if ref[m].size:
-                worst = max(worst, float(np.abs(blocks[m][b] - ref[m]).max()))
-    assert worst <= 1e-6
-    print(f"random set: {len(gt)} images, max |BEV, 3d overlap - oracle| = {worst:.3g}")
+        for m in range(3):
+            np.testing.assert_array_equal(blocks[m][b], ref[m])
     check_ap(ke.do_eval(gt, dt, [0, 1, 2], MO, True), ok.do_eval(gt, dt, [0, 1, 2], MO, True))
 
 
